@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the MMSSL hot training step on B200 (one process per GPU).
+"""Benchmark of the MMSSL hot training step on H100 (one process per GPU).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config baby] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config baby] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -17,6 +17,10 @@ triples per GPU per step.  Prints ONE JSON line (rank 0).
               vs the measured HBM peak in MEASURED_PEAKS.json.
   cpu_baseline / --impl reference : the oracle port of the reference's CPU path
               (oracle/mmssl_oracle.py, stock torch CPU ops, all host threads) on the same workload.
+  --dump-outputs DIR : after the timed steps, what the last device-resident step handed to its caller (loss terms,
+              gradients, updated parameters) as DIR/<name>.npy in float32, for output-for-output comparison of two builds.
+              The step is not bitwise reproducible (float-atomic heavy-row reductions, amplified by AdamW): two runs of the
+              same build agree to ~1e-5 in the loss terms and ~5e-3 in the gradients (DESIGN section 6).
 """
 from __future__ import annotations
 
@@ -67,6 +71,8 @@ def parse():
     ap.add_argument("--row-schedule", default="reduce_scatter", choices=["reduce_scatter", "allgather"],
                     help="products with a user-sized operand: partial products + reduce-scatter of the item-sized result, or all-gather of the operand")
     ap.add_argument("--row-graph", type=int, default=1, help="capture the row-sharded step in a CUDA graph (multicast exchange only)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs (loss terms, gradients, parameters) to DIR/<name>.npy (rank 0)")
     ap.add_argument("--graph-comm", action="store_true",
                     help="EXPERIMENTAL (hung in round 1): capture the DP all-reduce + AdamW inside the CUDA graph")
     return ap.parse_args()
@@ -78,7 +84,7 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -239,6 +245,35 @@ class HotStepTrainer:
         return float(self.pin_out[0])
 
 
+DUMP_BYTES = 64 * 1024 * 1024
+
+
+def step_outputs(trainer):
+    """Host copies of what one step of the timed path hands back: the five loss terms, the gradient of every live
+    parameter and the parameters after the optimiser step."""
+    from mmssl_b200.engine import LIVE
+    hs = trainer.hs
+    out = {"loss_terms": hs.out5.detach().float().cpu().numpy()}
+    for k in LIVE:
+        out["grad." + k] = hs.grads[k].detach().float().cpu().numpy()
+        out["param." + k] = hs.P[k].detach().float().cpu().numpy()
+    return out
+
+
+def dump_outputs(arrays, path):
+    """Writes every array as <path>/<name>.npy (float32).  Above DUMP_BYTES in all, the rows of each 2-D array are cut to
+    the same fixed, seeded sample (the same rows from run to run)."""
+    os.makedirs(path, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    keep = min(1.0, DUMP_BYTES / max(total, 1))
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        if keep < 1.0 and a.ndim == 2:
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], max(1, int(a.shape[0] * keep)), replace=False))
+            a = a[rows]
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def l2_flush(buf):
     buf.add_(1.0)
 
@@ -259,9 +294,9 @@ def roofline_objects(ds, P, feats, graphs, hbm_peak, peak_src, dev):
     """Time the two kernel classes that dominate the step, in isolation and with a cold L2."""
     from mmssl_b200 import ops
     d, I, U, nnz = ds.embed_size, ds.n_items, ds.n_users, ds.nnz
-    flush = torch.empty(192 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # 192 MiB > 126 MB L2
+    flush = torch.empty(192 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # 192 MiB > 50 MB L2
     out = {}
-    # --- projection GEMM (image modality, forward): tcgen05 + TMA, HBM-bound on reading F
+    # --- projection GEMM (image modality, forward): wgmma + TMA, HBM-bound on reading F
     fs = feats[0]
     w_hi, w_lo = ops.split_bf16(P["image_trans.weight"])
     floats, sk = ops.gemm_bf16x3_plan(I, d, fs.dim)
@@ -269,7 +304,7 @@ def roofline_objects(ds, P, feats, graphs, hbm_peak, peak_src, dev):
     ms = time_kernel(lambda: ops.gemm_bf16x3(fs.hi, fs.lo, w_hi, w_lo, I, d, fs.dim, sk, part), flush)
     alg = 4 * I * fs.dim + 4 * d * fs.dim + 4 * I * d
     gbs = alg / (ms * 1e-3) / 1e9
-    out["projection"] = {"kernel": f"gemm_bf16x3_kernel<{d}> (image_trans forward, tcgen05+TMA)", "bound": "hbm",
+    out["projection"] = {"kernel": f"gemm_bf16x3_kernel<{d}> (image_trans forward, wgmma+TMA)", "bound": "hbm",
                          "achieved": round(gbs, 1), "peak": hbm_peak, "unit": "GB/s", "frac": round(gbs / hbm_peak, 4),
                          "algorithmic_bytes": alg, "ms": round(ms, 5), "split_k": sk, "peak_source": peak_src,
                          "tflops_bf16_issued": round(3 * 2 * I * fs.dim * d / (ms * 1e-3) / 1e12, 2), "traffic": None}
@@ -286,17 +321,17 @@ def roofline_objects(ds, P, feats, graphs, hbm_peak, peak_src, dev):
                    "peak_source": peak_src, "traffic": None,
                    "note": "compulsory bytes are %.1f MB: at HBM peak that is %.1f us, below launch latency -> latency-bound at this scale"
                            % (alg / 1e6, alg / hbm_peak / 1e3)}
-    # `traffic` (dram__bytes of one launch) needs an ncu capture: it is never copied from a file here.  The captures of the same
-    # kernels are under profiles/ (see profiles/README.md); in-process it stays null.
+    # `traffic` (dram__bytes of one launch) needs an ncu capture (tools/spmm_large_ncu.py): it is never copied from a file here;
+    # in-process it stays null.
     out["library"] = library_kernels(ds, P, feats, graphs, x, y, flush, dev)
     del flush
     return out
 
 
 def library_kernels(ds, P, feats, graphs, x, y, flush, dev):
-    """The stock-torch kernels of the same two operators on this GPU, isolated, cold L2 (SURVEY 2.1: "the Blackwell-capable
-    kernel set to beat"): torch.sparse.mm on the reference's COO tensor (Models.py:69-73: coalesce + COO->CSR + cuSPARSE on every
-    call), the same on a prepared CSR tensor (cuSPARSE SpMM alone), and nn.Linear's fp32 cuBLAS GEMM (Models.py:173)."""
+    """The stock-torch kernels of the same two operators on this GPU, isolated, cold L2 (the library kernel set to beat):
+    torch.sparse.mm on the reference's COO tensor (Models.py:69-73: coalesce + COO->CSR + cuSPARSE on every call), the same
+    on a prepared CSR tensor (cuSPARSE SpMM alone), and nn.Linear's fp32 cuBLAS GEMM (Models.py:173)."""
     import torch.nn.functional as F
     from mmssl_b200 import ops
     out = {}
@@ -324,14 +359,14 @@ def library_kernels(ds, P, feats, graphs, x, y, flush, dev):
             ops.proj_epilogue(part, sk, I, d, b, None, yp)
         tf32 = torch.backends.cuda.matmul.allow_tf32
         torch.backends.cuda.matmul.allow_tf32 = False
-        out["projection"] = {"ours_ms (split W + tcgen05 GEMM + bias epilogue)": round(time_kernel(ours_proj, flush), 5),
+        out["projection"] = {"ours_ms (split W + wgmma GEMM + bias epilogue)": round(time_kernel(ours_proj, flush), 5),
                              "cublas_fp32_linear_ms": round(time_kernel(lambda: F.linear(fs.fp32, w, b), flush, reps=5), 5)}
         torch.backends.cuda.matmul.allow_tf32 = tf32
     return out
 
 
-CPU_THREADS_DEFAULT = 8      # fastest of {8,16,32,64,128} on the box's 128-thread Xeon 8562Y+: 0.37 s/step vs 40 s/step at 128
-                             # threads (profiles/r01_cpu_threads.txt) -- the baseline is reported at its best setting
+CPU_THREADS_DEFAULT = 8      # fastest of {8,16,32,64,128} on a 128-thread host (tools/cpu_threads.py): torch's CPU sparse kernels
+                             # slow down with more threads -- the baseline is reported at its best setting
 
 
 def cpu_baseline(name, seed, steps, batch, threads=0):
@@ -368,7 +403,7 @@ def cpu_baseline(name, seed, steps, batch, threads=0):
 
 
 def stock_gpu_baseline(name, seed, steps, warmup, batch, device, problem=None):
-    """SURVEY 8d's second comparator: what the unmodified reference's hot path costs on the same B200 through stock PyTorch
+    """SURVEY 8d's second comparator: what the unmodified reference's hot path costs on the same GPU through stock PyTorch
     (cuSPARSE / cuBLAS / ATen element-wise kernels, autograd, torch.optim.AdamW, one float(loss) sync per step like
     main.py:431) -- the restatement in oracle/mmssl_oracle.py run on CUDA tensors.  A comparator, not the product and not the
     target; timed with CUDA events around `steps` steps after `warmup`."""
@@ -443,7 +478,7 @@ def extra_config(name, a, dev, hbm_peak, peak_src):
     cfg = HotStepConfig(embed_size=d, n_layers=K, batch_size=BATCH, proj_impl=a.proj)
     trainer = HotStepTrainer(P, feats, graphs, cfg, BATCH, world=1)
     smp = TripleSampler(ds.train, seed=a.seed)
-    steps, warm = (200, 10) if nnz < 2_000_000 else (30, 5)
+    steps, warm = a.steps, a.warmup
     dev_batches = torch.from_numpy(np.stack([np.stack(smp.sample(BATCH)) for _ in range(16)])).to(dev)
     for w in range(warm):
         trainer.step_device(dev_batches[w % 16])
@@ -461,7 +496,8 @@ def extra_config(name, a, dev, hbm_peak, peak_src):
            "roofline_projection": roofs["projection"], "library_kernels": roofs["library"]}
     del trainer
     try:
-        sg = stock_gpu_baseline(name, a.seed, 20 if nnz < 2_000_000 else 5, 3, BATCH, str(dev), problem=cpu_problem)
+        # the comparator is a bounded sample of at most --steps steps (stock torch at 1M x 200k is ~10x slower than the step above)
+        sg = stock_gpu_baseline(name, a.seed, min(a.steps, 20 if nnz < 2_000_000 else 5), 3, BATCH, str(dev), problem=cpu_problem)
         out["stock_gpu"] = {"ms_per_step": sg["ms_per_step"], "value": sg["value"], "kind": sg["kind"], "speedup_ours": round(sg["ms_per_step"] / ms, 2)}
     except Exception as e:                      # the comparator must never take the bench line down (e.g. cuSPARSE out of memory)
         out["stock_gpu"] = {"unavailable": str(e)[:200]}
@@ -629,7 +665,7 @@ def row_shard_report(name, a, rank, world, dev):
         hs.masks = None
         hs.optimizer_step = True
         hs.capture(warmup=2)
-        n1 = 100 if nnz < 2_000_000 else 20
+        n1 = a.steps
         for s in range(3):
             hs.set_indices(*batches[s % 8]); hs.replay()
         torch.cuda.synchronize()
@@ -657,14 +693,14 @@ def row_shard_report(name, a, rank, world, dev):
             if rank == 0:
                 print(f"[bench] row-sharded step not captured ({e}); eager launches", file=sys.stderr)
     step = sh.replay if captured else sh.run
-    steps = 100 if nnz < 2_000_000 else 20
+    steps = a.steps
     for s in range(3):
         sh.set_indices(*batches[s % 8]); step()
     torch.cuda.synchronize()
     sh.n_gathers = sh.gathered_bytes = sh.n_reduce_scatters = 0
     # BEFORE the barrier: the query is a subprocess (~80 ms with 8 GPUs).  Between the barrier and the first event it made rank 0
     # enter the loop late while the other ranks' clocks were already running at their first exchange barrier: +75 ms / steps on
-    # the max over ranks (round 2: 8 GPUs, Sports 1.31 ms reported vs 0.57 ms measured by tools/rowshard_ab.py, 1M x 200k 11.7 vs ~7.9).
+    # the max over ranks.
     nv0 = nvlink_counters(dev.index) if rank == 0 else None
     dist.barrier()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -718,15 +754,13 @@ def main():
     config = {"workload": f"{a.config}: synthetic bipartite {U}x{I}, {nnz} edges, d={d}, {K}-layer GCN, V{dv}/T{dt} features, "
                           f"B={BATCH} triples per GPU per step, modality graphs alias ui/iu",
               "global_batch": BATCH * max(world, 1), "parallelism": "single GPU" if world == 1 else f"dp{world} (replicated graph, one flat gradient all-reduce per step" + (", captured in the CUDA graph)" if a.graph_comm else ", eager after the graph replay)"),
-              "l2_policy": "working set per step (%.0f MB of features) exceeds the 126 MB L2; isolated kernels timed after a 192 MiB L2 flush" % (4 * I * (dv + dt) / 1e6)}
+              "l2_policy": "working set per step (%.0f MB of features) exceeds the 50 MB L2; isolated kernels timed after a 192 MiB L2 flush" % (4 * I * (dv + dt) / 1e6)}
 
     if a.impl == "reference":
         if rank != 0:
             return
-        # bounded sample: a CPU hot step of this workload takes ~0.4 s at the best thread count; cap the run at ~1 minute
-        executed = max(1, min(a.steps, 100))
+        executed = max(1, a.steps)
         cb = cpu_baseline(a.config, a.seed, executed, BATCH, a.cpu_threads)
-        cb["sample"] += f" ({executed} of the requested {a.steps} steps executed: bounded sample)"
         line = {"impl": "reference", "metric": METRIC, "value": cb["value"], "unit": UNIT, "n_gpus": a.gpus, "steps": executed,
                 "warmup": 1, "ms_per_step": round(cb["s_per_step"] * 1e3, 3), "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": config, "cpu_baseline": cb,
@@ -737,8 +771,8 @@ def main():
     if a.impl == "stock-gpu":
         if rank != 0:
             return
-        sg = stock_gpu_baseline(a.config, a.seed, min(a.steps, 200), max(a.warmup, 3), BATCH, os.environ.get("MMSSL_STOCK_DEVICE", "cuda:0"))
-        print(json.dumps({"impl": "stock-torch-gpu", "metric": METRIC, "value": sg["value"], "unit": UNIT, "n_gpus": 1, "steps": min(a.steps, 200),
+        sg = stock_gpu_baseline(a.config, a.seed, a.steps, max(a.warmup, 3), BATCH, os.environ.get("MMSSL_STOCK_DEVICE", "cuda:0"))
+        print(json.dumps({"impl": "stock-torch-gpu", "metric": METRIC, "value": sg["value"], "unit": UNIT, "n_gpus": 1, "steps": a.steps,
                           "warmup": max(a.warmup, 3), "ms_per_step": sg["ms_per_step"], "higher_is_better": True, "dtype": "f32",
                           "data": "synthetic", "config": config, "comparator": sg}))
         return
@@ -752,6 +786,7 @@ def main():
     from mmssl_b200.hotstep import HotStepConfig
     from mmssl_b200.synthetic import TripleSampler
     _lib.load(require_device=True)
+    torch.manual_seed(a.seed + rank)     # the step's dropout masks come from torch's RNG: the same masks from run to run
     if a.spmm_impl is not None:
         ops.set_default_spmm_impl(a.spmm_impl)
 
@@ -801,6 +836,7 @@ def main():
     e1.record()
     barrier()
     ms_total = e0.elapsed_time(e1)
+    dumped = step_outputs(trainer) if a.dump_outputs and rank == 0 else None
     pts = [e0] + marks + [e1]
     seg_steps = [seg] * (n_seg - 1) + [a.steps - seg * (n_seg - 1)]
     seg_ms = [pts[i].elapsed_time(pts[i + 1]) / seg_steps[i] for i in range(n_seg)]
@@ -873,7 +909,8 @@ def main():
             line["row_shard"] = row_shard
         if world == 1:      # SURVEY 2.1 / 8d: the reference's own ops through stock torch on THIS GPU (comparator, not the product)
             try:
-                sg = stock_gpu_baseline(a.config, a.seed, 30, 5, BATCH, str(dev), problem=build_problem.last_cpu)
+                # the comparator is a bounded sample of at most --steps steps
+                sg = stock_gpu_baseline(a.config, a.seed, min(a.steps, 30), 5, BATCH, str(dev), problem=build_problem.last_cpu)
                 line["stock_gpu"] = {"ms_per_step": sg["ms_per_step"], "value": sg["value"], "kind": sg["kind"], "sample": sg["sample"],
                                      "speedup_ours": round(sg["ms_per_step"] / (ms_total / a.steps), 2)}
             except Exception as e:
@@ -908,6 +945,8 @@ def main():
                         line["configs"][name] = {"failed": repr(e)[:300]}
         if not a.no_cpu_baseline and world == 1:
             line["cpu_baseline"] = cpu_baseline(a.config, a.seed, a.cpu_steps, BATCH, a.cpu_threads)
+        if dumped is not None:
+            dump_outputs(dumped, a.dump_outputs)
         print(json.dumps(line))
         if parity is not None and not parity["ok"]:
             print("[bench] N-GPU vs 1-GPU parity FAILED: " + json.dumps(parity), file=sys.stderr)

@@ -1,4 +1,4 @@
-/* mmssl_b200 -- C ABI of the B200-native MMSSL hot path (libmmssl_b200.so, sm_100a only).
+/* mmssl_b200 -- C ABI of the H100-native MMSSL hot path (libmmssl_b200.so, sm_90a only).
  *
  * Plain pointers and sizes; no torch types.  Every pointer is a DEVICE pointer unless it is a
  * small descriptor struct/array marked "host".  `stream` is a cudaStream_t passed as void*.
@@ -7,7 +7,7 @@
  * row-major fp32 with an explicit leading dimension (in floats).
  *
  * Each entry point names the reference code it replaces (paths relative to
- * /root/reference/MMSSL/).  The reference itself is Python on stock torch ops, so the
+ * MMSSL/ of the reference repository).  The reference itself is Python on stock torch ops, so the
  * "reference-side binding" is the ctypes stub in mmssl_b200/_lib.py (see INTEGRATION.md).
  */
 #ifndef MMSSL_B200_H
@@ -24,7 +24,7 @@ extern "C" {
 
 int mmssl_abi_version(void);
 const char* mmssl_last_error(void);
-/* 0 if the current device is compute capability 10.x (B200); fails loudly otherwise. */
+/* 0 if the current device is compute capability 9.x (H100); fails loudly otherwise. */
 int mmssl_device_check(void);
 
 /* ------------------------------------------------------------------ graph preparation
@@ -142,7 +142,7 @@ int mmssl_reduce_rows_epilogue(int64_t n_rows, int d, int nrhs, const mmssl_spmm
 int mmssl_sgemm(int trans_a, int trans_b, int64_t m, int64_t n, int64_t k, float alpha, const float* a, int64_t lda,
                 const float* b, int64_t ldb, float beta, float* c, int64_t ldc, int split_k, void* stream);
 
-/* ------------------------------------------------------------------ projection (tcgen05 + TMA)
+/* ------------------------------------------------------------------ projection (wgmma + TMA)
  * X = F * W^T + b  and  dW = dX^T * F, fp32 semantics via a bf16 hi/lo split (3 MMAs per product),
  * replaces nn.Linear image_trans/text_trans forward and weight gradient (Models.py:28-31,173-174).
  * Declared in the "projection" section below once built (mmssl_proj_*). */
@@ -220,9 +220,9 @@ int mmssl_infonce_stats(const float* a, const float* b, int64_t n, int d, float 
 int mmssl_infonce_grad(const float* a, const float* b, int64_t n, int d, float inv_tau, const float* coef, float* ga,
                        float* gb, void* stream);
 /* through the normalisation, then (atomic) scatter-add into the tables: g_z1[idx[i]] += ..., g_z2[idx[i]] += ... */
-/* Tensor-core InfoNCE for n <= 2048, d in {64, 128} (loss_tc.cu): the similarity tiles a a^T, a b^T on tcgen05 (bf16 hi/lo, three
- * MMAs per product), exp / row sums / diagonal in the TMEM epilogue, the exponentials kept as bf16 hi/lo matrices in `workspace`;
- * the backward = three split-K tcgen05 products of those matrices with [a | u.a], b, u.a + one combine kernel.  Same inputs and
+/* Tensor-core InfoNCE for n <= 2048, d in {64, 128} (loss_tc.cu): the similarity tiles a a^T, a b^T on wgmma (bf16 hi/lo, three
+ * MMAs per product), exp / row sums / diagonal in the register epilogue, the exponentials kept as bf16 hi/lo matrices in `workspace`;
+ * the backward = three split-K wgmma products of those matrices with [a | u.a], b, u.a + one combine kernel.  Same inputs and
  * outputs as mmssl_infonce_stats / mmssl_infonce_grad (ga, gb are WRITTEN here, accumulated there). */
 int mmssl_infonce_tc_supported(int64_t n, int d);
 int64_t mmssl_infonce_tc_workspace_bytes(int64_t n, int d);
@@ -382,7 +382,7 @@ int mmssl_topk_rows(const float* x, int64_t ldx, int64_t rows, int64_t w, int k,
 int mmssl_pair_append(const int64_t* users, int64_t batch, const int64_t* ids, int k, int64_t* x, int64_t* y, void* stream);
 int mmssl_degree_values(const int64_t* idx, int64_t n, int64_t n_rows, int32_t* deg_scratch, float* vals, void* stream);
 
-/* ------------------------------------------------------------------ projection (tcgen05 + TMA), see proj_tc.cu */
+/* ------------------------------------------------------------------ projection (wgmma + TMA), see proj_tc.cu */
 int mmssl_split_bf16(const float* x, int64_t ldx, int64_t rows, int64_t cols, uint16_t* hi, uint16_t* lo, int64_t ldo,
                      void* stream);
 /* transposed split: hi/lo [cols][ldo] from x [rows][cols] (optionally multiplied by mask [rows][cols]) */
@@ -403,7 +403,7 @@ int mmssl_gemm_bf16x3(const uint16_t* a_hi, const uint16_t* a_lo, int64_t lda, c
 int mmssl_gemm_bf16x3_wide(const uint16_t* a_hi, const uint16_t* a_lo, int64_t lda, const uint16_t* b_hi,
                            const uint16_t* b_lo, int64_t ldb, int64_t m, int64_t n, int64_t k, float alpha, int accumulate,
                            float* c, int64_t ldc, void* stream);
-/* Tuning / test knob of the kernel above: k-blocks (64 of K each) chained into one TMEM accumulator before the epilogue folds
+/* Tuning / test knob of the kernel above: k-blocks (64 of K each) chained into one accumulator before the epilogue folds
  * the pass into C with fp32 adds (default 16 = 1024 of K; bounds the tensor core's accumulation error, gemm_wide.cu). */
 int mmssl_gemm_wide_set_chunk(int k_blocks);
 /* y[m][ldy + col_off] = (sum_s partial[s][m][n] + bias[n]) * mask[m][n]     (bias / mask may be NULL) */

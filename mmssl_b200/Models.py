@@ -4,8 +4,8 @@
 ``forward`` signatures, same registered parameter names (state_dict compatible), same module-global
 ``args`` convention (Models.py:13-15), same 12-tuple with outputs 0/6 and 1/7 being the same objects
 (Models.py:220).  What changes is what runs: ``forward`` is ONE autograd node whose forward and
-backward are the sm_100a kernels of libmmssl_b200 (functional.MMSSLForwardFn) -- CSR SpMM with fused
-softmax / layer-sum epilogues, tcgen05 projection, fused row-wise glue.  There is no eager fallback.
+backward are the sm_90a kernels of libmmssl_b200 (functional.MMSSLForwardFn) -- CSR SpMM with fused
+softmax / layer-sum epilogues, wgmma projection, fused row-wise glue.  There is no eager fallback.
 
 ``Discriminator`` stays a stock-torch module with the reference's architecture so that the reference's own trainer and its
 checkpoints keep working; the device implementation of the GAN side (no autograd) is mmssl_b200/gan.py + fullstep.py, which

@@ -1,4 +1,4 @@
-"""mmssl_b200 -- the MMSSL training step (HKUDS/MMSSL) on B200, hand-written CUDA behind a C ABI.
+"""mmssl_b200 -- the MMSSL training step (HKUDS/MMSSL) on H100, hand-written CUDA behind a C ABI.
 
   Models          drop-in for the reference's Models.py (MMSSL as one autograd node, Discriminator)
   functional      autograd wrappers: SpMMFunction, bpr_loss, batched_contrastive_loss, feat_reg_loss
@@ -13,7 +13,7 @@
   parallel        data-parallel bucket / fused multimem optimiser, row-sharded propagation, symmetric tables
   rowshard_step   the whole hot step under the row-sharded scheme (NCCL or multicast exchange)
   graph, ops, _lib   prepared sparse operands, tensor-level wrappers, ctypes binding of libmmssl_b200.so
-  build           nvcc build of the library (sm_100a)
+  build           nvcc build of the library (sm_90a)
 
 Nothing is imported here: `import mmssl_b200` stays cheap, every sub-module loads the library on first use and refuses to run
-without it and a B200 (no CPU or eager-PyTorch fallback)."""
+without it and an H100 (no CPU or eager-PyTorch fallback)."""

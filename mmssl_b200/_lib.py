@@ -2,7 +2,7 @@
 
 This is the "reference-side binding" of the drop-in: the reference is Python, so the FFI a
 maintainer would add is this ctypes stub.  The library is the ONLY compute back-end: if it is
-missing, or the device is not a B200, loading fails loudly -- there is no CPU / eager fallback.
+missing, or the device is not an H100, loading fails loudly -- there is no CPU / eager fallback.
 """
 from __future__ import annotations
 
@@ -186,7 +186,7 @@ def load(require_device: bool = False) -> C.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise MmsslLibraryError(
-                f"{LIB_PATH} is missing: build it with `python -m mmssl_b200.build` (nvcc, sm_100a). "
+                f"{LIB_PATH} is missing: build it with `python -m mmssl_b200.build` (nvcc, sm_90a). "
                 "mmssl_b200 has no CPU or eager-PyTorch fallback.")
         lib = C.CDLL(LIB_PATH)
         missing = []
@@ -207,7 +207,7 @@ def load(require_device: bool = False) -> C.CDLL:
         _lib = lib
     if require_device:
         if not torch.cuda.is_available():
-            raise MmsslLibraryError("mmssl_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise MmsslLibraryError("mmssl_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         check(_lib.mmssl_device_check())
     return _lib
 

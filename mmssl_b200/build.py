@@ -1,4 +1,4 @@
-"""Build libmmssl_b200.so in-tree with nvcc for sm_100a (no torch extension machinery: the library
+"""Build libmmssl_b200.so in-tree with nvcc for sm_90a (no torch extension machinery: the library
 is a plain C-ABI shared object, loaded with ctypes).
 
     python -m mmssl_b200.build [--force] [--verbose]
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libmmssl_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function",
          "--expt-relaxed-constexpr", "--expt-extended-lambda", "-Xptxas", "-warn-spills"]
 

@@ -1,4 +1,4 @@
-// Shared helpers for the mmssl_b200 CUDA library (sm_100a only).
+// Shared helpers for the mmssl_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -32,7 +32,7 @@ int fail_cuda(const char* where, cudaError_t e);
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-constexpr int kNumSMs = 148;   // B200
+constexpr int kNumSMs = 132;   // H100 SXM
 
 // ---- programmatic dependent launch (PDL) ----
 // Kernels on the critical path of the captured step are launched with

@@ -29,6 +29,6 @@ extern "C" int mmssl_device_check(void) {
     MMSSL_CUDA(cudaGetDevice(&dev));
     int major = 0;
     MMSSL_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    MMSSL_REQUIRE(major == 10, "libmmssl_b200 is built for sm_100a (B200) only; no other device and no CPU fallback");
+    MMSSL_REQUIRE(major == 9, "libmmssl_b200 is built for sm_90a (H100) only; no other device and no CPU fallback");
     return 0;
 }

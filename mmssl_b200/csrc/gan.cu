@@ -7,7 +7,7 @@
 // The GEMMs between them go through the library's GEMM entry points.  All of this is HBM-bound reduction work on
 // [2B, I/4], [2B, I/8] and [B, I] fp32 tiles (I/4 is not a multiple of 4 in general, so loads are scalar and coalesced
 // along the row).  Two kernel shapes:
-//   * column ops  -- CTA = 8 columns x 32 row lanes (h = I/4 = 1762 at Baby gives 221 CTAs: the 148 SMs are covered, which a
+//   * column ops  -- CTA = 8 columns x 32 row lanes (h = I/4 = 1762 at Baby gives 221 CTAs: the 132 SMs are covered, which a
 //                    32-column CTA would not do); a column's statistics are reduced in a fixed order (deterministic);
 //                    multi-pass kernels re-read their 8-column stripe from L2.
 //   * row ops     -- one CTA (256 threads) or one warp per row, block reductions in a fixed order.

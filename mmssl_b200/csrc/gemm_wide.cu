@@ -5,26 +5,23 @@
 // The Discriminator's first layer (Models.py:224-245, nn.Linear(n_items, n_items/4)) makes every D call of the reference's
 // iteration a [2B, I] x [I, I/4] product, and the closed-form backward / gradient-penalty sweeps (oracle/gan_oracle.py) add
 // its transposed variants: 11 such products per iteration (Baby: 2048 x 7050 x 1762 = 50.9 GFLOP each).  Compute-bound:
-// tcgen05, with the same bf16 hi/lo operand split as the projection (fp32 contract, 1e-4 relative), i.e. 3 MMAs per product.
+// wgmma, with the same bf16 hi/lo operand split as the projection (fp32 contract, 1e-4 relative), i.e. 3 MMAs per product.
 //
-// Same anatomy as proj_tc.cu (warp 0 = TMA producer, warp 1 = TMEM alloc + single-thread MMA issuer, warps 2-5 = epilogue),
-// but tiled over N as well: CTA (m_tile, n_tile) owns a 128 x NT tile of C for the whole K range (no split-K: every
-// shape on this path gives >= 100 tiles).
+// Same anatomy as proj_tc.cu (two consumer warpgroups with register accumulators, one TMA producer warp, tc_common.cuh), but
+// tiled over N as well: CTA (m_tile, n_tile) owns a 128 x NT tile of C for the whole K range (no split-K: every shape on this
+// path gives >= 100 tiles).
 //
 // Accumulation length is bounded: the tensor core's fp32 accumulate is not round-to-nearest, so its error grows with the
-// number of MMAs chained into one TMEM accumulator (round 1 on hardware: K = 7050 in one pass -> 2.8e-5 max-norm error, while
-// the split-K projection kernel stays under 1e-5 at the same K).  The K range is therefore cut into passes of `chunk_kb`
-// k-blocks (default 16 = 1024 of K = 192 chained MMAs); each pass accumulates into one of TWO TMEM buffers (2 x NT columns)
-// and the epilogue warps fold a finished pass into C with round-to-nearest fp32 adds (C (+)= alpha * pass; C is L2-resident)
-// while the MMA warp is already filling the other buffer.  Both operands are re-read from L2 by the other tiles of their row / column of the grid, so both are
-// hinted evict-last (the policy constant proj_tc.cu already uses on hardware).  Rows / columns beyond m / n: TMA zero-fills the loads, the epilogue masks the stores;
-// C's leading dimension is arbitrary (I/4 is not a multiple of 4), 128-bit stores are used when the row is aligned.
+// number of MMAs chained into one accumulator.  The K range is therefore cut into passes of `chunk_kb` k-blocks (default 16 =
+// 1024 of K = 192 chained MMAs); after each pass the consumer warps fold the accumulator into C with round-to-nearest fp32 adds
+// (C (+)= alpha * pass; C is L2-resident) and start the next pass from zero.  Both operands are re-read from L2 by the other
+// tiles of their row / column of the grid, so both are hinted evict-last.  Rows / columns beyond m / n: TMA zero-fills the
+// loads, the epilogue masks the stores; C's leading dimension is arbitrary (I/4 is not a multiple of 4): column pairs are stored
+// as 8-byte accesses when ldc is even, element by element otherwise.
 //
-// Executed on the CPU through a functional model
-// of the PTX it issues (tests/cuemu/cuemu_ptx.cpp, calibrated on proj_tc.cu which is green on hardware; tests/test_emu_tensor_core.py:
-// multi-tile N, ragged edges, both epilogues; a wrong TMA coordinate, barrier phase or epilogue row mapping is caught there).
-// Its GPU test (tests/test_gpu_zzz_gemm_wide.py, sorts last) runs with the suite; mmssl_b200.gan_ops keeps the fp32 CUDA-core GEMM
-// as default until that test has passed on a B200.  mbar_wait traps instead of hanging.
+// Executed on the CPU through a functional model of the PTX it issues (tests/cuemu/cuemu_ptx.cpp; tests/test_emu_tensor_core.py:
+// multi-tile N, ragged edges, both epilogues, several passes); its GPU test is tests/test_gpu_zzz_gemm_wide.py.  mbar_wait traps
+// instead of hanging.
 #include "tc_common.cuh"
 #include "../../include/mmssl_b200.h"
 
@@ -37,8 +34,6 @@ struct WideCfg {
     static constexpr int kStageBytes = 2 * kTileABytes + 2 * kTileBBytes;      // 96 KB at NT = 256, 64 KB at NT = 128
     static constexpr int kStages = (NT == 256) ? 2 : 3;
     static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-    static constexpr uint32_t kIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NT >> 3) << 17) |
-                                       ((uint32_t)(kBlockM >> 4) << 24);       // F32 acc, BF16 x BF16, K-major both
 };
 
 template <int NT>
@@ -51,35 +46,21 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
     uint64_t* empty_bar = full_bar + Cfg::kStages;
-    uint64_t* acc_full = empty_bar + Cfg::kStages;      // [2]: a pass is complete in TMEM buffer b
-    uint64_t* acc_empty = acc_full + 2;                 // [2]: the epilogue warps have drained buffer b
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m_tile = blockIdx.x, n_tile = blockIdx.y;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_a_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_a_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b_lo) : "memory");
+        for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-            for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 4); }
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(2 * NT) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         if (lane == 0) {
             for (int i = 0; i < nkb; ++i) {
                 const int s = i % Cfg::kStages;
@@ -94,87 +75,40 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
                 tma_load_2d(&tm_b_lo, &full_bar[s], st + 2 * kTileABytes + Cfg::kTileBBytes, kx, n_tile * NT, kEvictLast);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            for (int i = 0; i < nkb; ++i) {
-                const int s = i % Cfg::kStages;
-                const uint32_t ph = (uint32_t)(i / Cfg::kStages) & 1u;
-                const int pass = i / chunk_kb, j = i - pass * chunk_kb, b = pass & 1;
-                if (j == 0) {                       // buffer b was last used by pass - 2: wait until it has been drained
-                    mbar_wait(&acc_empty[b], (((uint32_t)(pass >> 1)) & 1u) ^ 1u);
-                    tc_fence_after();
-                }
-                const uint32_t tmem_acc = tmem_base + (uint32_t)(b * NT);
-                mbar_wait(&full_bar[s], ph);
-                tc_fence_after();
-                const uint32_t a_hi = smem_u32(smem + s * Cfg::kStageBytes);
-                const uint32_t a_lo = a_hi + kTileABytes;
-                const uint32_t b_hi = a_hi + 2 * kTileABytes;
-                const uint32_t b_lo = b_hi + Cfg::kTileBBytes;
-#pragma unroll
-                for (int k = 0; k < kBlockK / 16; ++k) {
-                    const uint32_t off = k * 32;   // 16 bf16 = 32 bytes inside the 128-byte swizzle span
-                    const uint64_t dah = make_sw128_kmajor_desc(a_hi + off), dal = make_sw128_kmajor_desc(a_lo + off);
-                    const uint64_t dbh = make_sw128_kmajor_desc(b_hi + off), dbl = make_sw128_kmajor_desc(b_lo + off);
-                    umma_bf16(tmem_acc, dah, dbh, Cfg::kIdesc, (j > 0 || k > 0) ? 1u : 0u);
-                    umma_bf16(tmem_acc, dah, dbl, Cfg::kIdesc, 1u);
-                    umma_bf16(tmem_acc, dal, dbh, Cfg::kIdesc, 1u);
-                }
-                umma_commit(&empty_bar[s]);   // frees the smem stage once the MMAs have read it
-                if (j == chunk_kb - 1 || i == nkb - 1) umma_commit(&acc_full[b]);   // this pass is complete
-            }
-        }
     } else {
-        const int q = warp & 3;               // TMEM lane quarter this warp may access
-        const int64_t row = (int64_t)m_tile * kBlockM + q * 32 + lane;
+        const int64_t row0 = (int64_t)m_tile * kBlockM + 64 * (warp >> 2);
         const int col0 = n_tile * NT;
-        float* out = C + row * ldc + col0;
-        const bool row_ok = row < M;
-        const bool vec_ok = row_ok && ((reinterpret_cast<uintptr_t>(out) & 15u) == 0);
+        const bool pair_ok = (ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(C) & 7u) == 0;   // every (row, even col) pair 8-byte aligned
         const int n_pass = (nkb + chunk_kb - 1) / chunk_kb;
+        float acc[NT / 2];
         for (int pass = 0; pass < n_pass; ++pass) {
-            const int b = pass & 1;
             const bool add_c = accumulate != 0 || pass > 0;       // later passes fold into what the earlier ones stored
-            mbar_wait(&acc_full[b], ((uint32_t)(pass >> 1)) & 1u);
-            tc_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < NT; c += 32) {
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(b * NT + c), v);     // warp-collective: every lane executes it
-                if (!row_ok || col0 + c >= Ntot) continue;
-                if (vec_ok && col0 + c + 32 <= Ntot) {
-                    float4 prev[8];
+#pragma unroll
+            for (int j = 0; j < NT / 2; ++j) acc[j] = 0.f;
+            mma_kblocks<NT, Cfg::kStages, Cfg::kStageBytes>(acc, smem, full_bar, empty_bar, pass * chunk_kb, min(nkb, (pass + 1) * chunk_kb));
+#pragma unroll
+            for (int j = 0; j < NT / 2; j += 2) {         // acc[j], acc[j + 1]: columns col, col + 1 of one row
+                const int64_t row = row0 + frag_row(warp, lane, j);
+                const int col = col0 + frag_col(lane, j);   // even
+                if (row >= M || col >= Ntot) continue;
+                float* out = C + row * ldc + col;
+                if (pair_ok && col + 1 < Ntot) {            // 8-byte access: a lane quad covers 32 contiguous bytes of the row
+                    float2 r = make_float2(alpha * acc[j], alpha * acc[j + 1]);
                     if (add_c) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) prev[j] = ld4(out + c + 4 * j);
+                        const float2 prev = *reinterpret_cast<const float2*>(out);
+                        r.x += prev.x;
+                        r.y += prev.y;
                     }
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        float4 r = make_float4(alpha * __uint_as_float(v[4 * j]), alpha * __uint_as_float(v[4 * j + 1]),
-                                               alpha * __uint_as_float(v[4 * j + 2]), alpha * __uint_as_float(v[4 * j + 3]));
-                        if (add_c) r = add4(r, prev[j]);
-                        st4(out + c + 4 * j, r);
-                    }
+                    *reinterpret_cast<float2*>(out) = r;
                 } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        if (col0 + c + j < Ntot) {
-                            float r = alpha * __uint_as_float(v[j]);
-                            if (add_c) r += out[c + j];
-                            out[c + j] = r;
-                        }
+                    for (int e = 0; e < 2 && col + e < Ntot; ++e) {
+                        float r = alpha * acc[j + e];
+                        if (add_c) r += out[e];
+                        out[e] = r;
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[b]);            // 4 epilogue warps -> the MMA warp may overwrite buffer b
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(2 * NT) : "memory");
     }
 }
 
@@ -198,7 +132,7 @@ static int launch_wide(const CUtensorMap& ah, const CUtensorMap& al, const CUten
 
 using namespace mmssl;
 
-// k-blocks (64 of K each) chained into one TMEM accumulator before the epilogue folds it into C (see the file header).
+// k-blocks (64 of K each) chained into one accumulator before the epilogue folds it into C (see the file header).
 static int g_wide_chunk_kb = 16;
 
 extern "C" int mmssl_gemm_wide_set_chunk(int k_blocks) {

@@ -91,7 +91,7 @@ static cudaError_t carve_csr_ws(int64_t nnz, int64_t n_rows, void* base, CsrWs* 
 // Heavier rows (the head of a power-law degree distribution): segments of 64 that accumulate with
 // 128-bit float atomics into a dedicated zeroed row -- a serial reduction over hundreds of partials
 // would otherwise be the kernel's critical path.  (Summation order of those few rows is not fixed.)
-// Defaults from the round-2 measurement (tools/probe.py plan): the kernel's duration on a small graph is its longest item --
+// Defaults chosen by measurement on the earlier hardware (tools/probe.py plan; not re-tuned for the H100): the kernel's duration on a small graph is its longest item --
 // an item of 64 non-zeros is 8 dependent gather batches of 8 -- so rows are cut earlier than the first version did (64 / 32).
 struct PlanCuts { int split_threshold, seg_len, heavy_threshold, heavy_seg_len; };
 static PlanCuts g_cuts = {64, 32, 1024, 64};

@@ -7,10 +7,10 @@
 // Each block owns a tile of TR = 32 or 64 rows and runs register-tiled (4x4 per thread) products against the
 // d x d matrix staged in shared memory, with the row-wise normalisation / its backward fused as
 // prologue / epilogue.  (A first version walked rows one by one and re-read the whole matrix from
-// shared memory per row: shared-memory-bandwidth bound, 16-34 us; this one is ~4x faster.)
+// shared memory per row: shared-memory-bandwidth bound.)
 // Shared memory is 24 KB per block at d = 64 (matrix 16 KB + one 8 KB row tile; the backward keeps its second tile in the
-// matrix's place until the matrix is needed): these kernels run beside the projection GEMMs, whose two 99.5 KB CTAs leave 27 KB
-// of an SM -- with 32 / 48 KB blocks they waited for the GEMM to drain (round-2 trace: 29-44 us instead of 10-17).
+// matrix's place until the matrix is needed): these kernels run beside the projection GEMMs, whose two ~97 KB CTAs leave ~30 KB
+// of an SM -- with 32 / 48 KB blocks they would wait for the GEMM to drain.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(TR * 4) id_fuse2_bwd_kernel(const float* __res
 
 // dWcat[h*d*d + i] = sum over the partial tiles of both sides (fixed order), for every head h.
 // block = 32 outputs x 32 slices of the partial-tile list (a slice walks its ~26 tiles of Baby's 829 in batches of 8 independent
-// loads); slices are combined in order.  (First version: 64 outputs x 4 slices, 13 dependent batches per thread, 7.7 us.)
+// loads); slices are combined in order.  (A first version used 64 outputs x 4 slices: 13 dependent batches per thread.)
 constexpr int kRedOut = 32, kRedSlices = 32;
 __global__ void __launch_bounds__(kRedOut * kRedSlices) dwcat_reduce_kernel(const float* __restrict__ part_u, int nu,
                                                                             const float* __restrict__ part_i, int ni, int d, int heads,
@@ -286,7 +286,7 @@ extern "C" int mmssl_wsum(const float* wcat, int d, int heads, float* wsum, floa
 }
 
 static int idfuse_carveout() {          // percent of the SM's L1 / shared array; MMSSL_IDFUSE_CARVEOUT: experiment knob
-    const char* e = getenv("MMSSL_IDFUSE_CARVEOUT");       // (asking for the GEMMs' configuration, 100, changed nothing: round-2 call x3)
+    const char* e = getenv("MMSSL_IDFUSE_CARVEOUT");       // (asking for the GEMMs' configuration, 100, changed nothing on the earlier hardware)
     return e ? atoi(e) : (int)cudaSharedmemCarveoutDefault;
 }
 

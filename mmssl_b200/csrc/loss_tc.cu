@@ -2,22 +2,21 @@
 //
 // For a batch of n <= 2048 rows the two similarity matrices  a a^T  and  a b^T  (a = normalised z1 rows, b = normalised z2 rows)
 // are n x n x d contractions: 0.27 GFLOP at n = 1024, d = 64 -- tensor-core work.  The fp32 contract (1e-4) is kept the way the
-// projection keeps it: operands as bf16 hi + lo pairs, three MMAs per product, fp32 accumulation in TMEM (K = d <= 256: 48
+// projection keeps it: operands as bf16 hi + lo pairs, three MMAs per product, fp32 accumulation in registers (K = d <= 256: 48
 // chained MMAs at most, far below the lengths where the accumulate error shows, gemm_wide.cu).  |s / tau| <= 2, so a 1e-5
 // error in s is 2e-5 in exp(s / tau).
 //
 //   forward  nce_stats_tc_kernel: CTA (it, jt, m) owns ONE 128 x 128 tile of  S_R = A_i A_j^T (m = 0),  S_B = A_i B_j^T (1)  or
-//            S_T = B_i A_j^T (2: the transposed block of a b^T that the backward needs row-major) in a TMEM accumulator -- 192 CTAs
-//            at n = 1024, two per SM, all resident at once (the first version kept the three tiles in one CTA: 64 CTAs on 148 SMs,
-//            21.7 us, epilogue-bound); operands by TMA
-//            (SWIZZLE_128B), single-thread tcgen05.mma issue, eight epilogue warps: tcgen05.ld -> exp -> row sums, diagonal,
-//            and the exponentials themselves stored as bf16 hi / lo matrices E_R, E_B, E_T (12 MB at n = 1024: L2-resident).
+//            S_T = B_i A_j^T (2: the transposed block of a b^T that the backward needs row-major) in the registers of its two
+//            wgmma warpgroups -- 192 CTAs at n = 1024, two per SM; operands by TMA (SWIZZLE_128B); the same warps then compute
+//            exp -> row sums, diagonal, and the exponentials themselves stored as bf16 hi / lo matrices E_R, E_B, E_T (12 MB at
+//            n = 1024: L2-resident).
 //            nce_finalize_kernel (loss.cu) turns the sums into loss rows and backward coefficients u, v as before.
 //   backward with P_ij = -(u_i + u_j) R_ij / tau (i != j), Q_ij = B_ij (-u_i + [i == j] v_i) / tau:
 //              dL/da_i = sum_j P_ij a_j + Q_ij b_j = -(1/tau) [ u_i (E_R a)_i + (E_R (u.a))_i + u_i (E_B b)_i ] + diagonal terms
 //              dL/db_j = sum_i Q_ij a_i           = -(1/tau) (E_T (u.a))_j + diagonal term
 //            i.e. three products of the stored exponentials with [a | u.a], b and u.a: nce_operands_kernel writes those operands
-//            transposed (K-major over the batch) as bf16 hi / lo, the products run on the projection's split-K tcgen05 kernel
+//            transposed (K-major over the batch) as bf16 hi / lo, the products run on the projection's split-K wgmma kernel
 //            (mmssl_gemm_bf16x3), nce_combine_kernel sums the K slices and applies the coefficients.
 // Larger batches (B = 16384: the exponentials would take 3 TB) and d = 256 (operand width 512) stay on the CUDA-core kernels.
 #include <cuda_bf16.h>
@@ -33,10 +32,9 @@ int nce_prepare_split_launch(const float* z1, int64_t ldz1, const float* z2, int
 
 constexpr int kNceTile = 128;
 constexpr int kNceMaxN = 2048;
-constexpr uint32_t kNceIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kNceTile >> 3) << 17) | ((uint32_t)(kBlockM >> 4) << 24);
 constexpr int kNceStageBytes = 4 * kTileABytes;                     // row operand, column operand  x  hi, lo : 64 KB
-constexpr int kNceRows = 32, kNceRowPitch = 144;                    // epilogue staging: 32 rows x (128 B + 16 B pad) per warp, hi and lo
-constexpr int kNceEpiBytes = 8 * 2 * kNceRows * kNceRowPitch;       // 72 KB, laid over the operand tiles (dead once the MMAs completed)
+constexpr int kNceRows = 16, kNceRowPitch = 272;                    // epilogue staging: a warp's 16 rows x (256 B + 16 B pad), hi and lo
+constexpr int kNceEpiBytes = kConsumerWarps * 2 * kNceRows * kNceRowPitch;   // 68 KB, laid over the operand tiles (dead once the MMAs completed)
 constexpr int kNceSmemBytes = kNceEpiBytes + 256 + 1024;            // 2 CTAs per SM
 
 // bf16 pair (x in the low half) with one cvt.rn.bf16x2; its two halves widened back to fp32 are shifts
@@ -50,36 +48,8 @@ __device__ __forceinline__ float fast_exp2(float x) {      // MUFU.EX2: |x| <= 2
     return y;
 }
 
-// 32 accumulator columns of one row -> exponentials (bf16 hi / lo pairs) and their sum.  CHECK: rows / columns beyond n give 0 and
-// the diagonal element (row i == column) is stored to diag[i].
-template <bool CHECK>
-__device__ __forceinline__ float nce_exp32(const uint32_t (&v)[32], float scale, int64_t i, int64_t jbase, int64_t n, float* diag,
-                                           uint32_t (&ph)[16], uint32_t (&pl)[16]) {
-    float part = 0.f;
-#pragma unroll
-    for (int t = 0; t < 32; t += 2) {
-        float e0, e1;
-        if (CHECK) {
-            e0 = (i < n && jbase + t < n) ? fast_exp2(__uint_as_float(v[t]) * scale) : 0.f;
-            e1 = (i < n && jbase + t + 1 < n) ? fast_exp2(__uint_as_float(v[t + 1]) * scale) : 0.f;
-            if (diag != nullptr && i < n) {
-                if (i == jbase + t) diag[i] = e0;
-                if (i == jbase + t + 1) diag[i] = e1;
-            }
-        } else {
-            e0 = fast_exp2(__uint_as_float(v[t]) * scale);
-            e1 = fast_exp2(__uint_as_float(v[t + 1]) * scale);
-        }
-        part += e0 + e1;
-        const uint32_t hp = pack_bf16(e0, e1);
-        ph[t / 2] = hp;
-        pl[t / 2] = pack_bf16(e0 - __uint_as_float(hp << 16), e1 - __uint_as_float(hp & 0xffff0000u));
-    }
-    return part;
-}
-
 // stats layout (loss.cu): [diagR n][diagB n][loss n][unused n][partR ntj*n][partB ntj*n],  ntj = 2 * gridDim.y
-constexpr int kNceThreads = 320;       // warp 0 TMA producer, warp 1 MMA issuer + TMEM owner, warps 2-9 epilogue
+constexpr int kNceThreads = kThreads;   // warps 0-7 two wgmma warpgroups + epilogue, warp 8 TMA producer
 
 __global__ void __launch_bounds__(kNceThreads, 2)
 nce_stats_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
@@ -90,33 +60,22 @@ nce_stats_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
     static_assert(kNceEpiBytes >= kNceStageBytes, "staging lies over the operand tiles");
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kNceEpiBytes);
     uint64_t* empty_bar = full_bar + 1;
-    uint64_t* accum_bar = empty_bar + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int it = blockIdx.x, jt = blockIdx.y;
     const int mat = blockIdx.z;                                   // 0: S_R = A_i A_j^T   1: S_B = A_i B_j^T   2: S_T = B_i A_j^T
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_a_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_a_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b_lo) : "memory");
+        mbar_init(full_bar, 1); mbar_init(empty_bar, kConsumerWarps);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        if (lane == 0) {
-            mbar_init(full_bar, 1); mbar_init(empty_bar, 1); mbar_init(accum_bar, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(128) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    float acc[kNceTile / 2];
+    if (warp == kProducerWarp) {
         if (lane == 0) {
             for (int kb = 0; kb < nkb; ++kb) {
                 mbar_wait(empty_bar, ((uint32_t)kb & 1u) ^ 1u);
@@ -132,79 +91,73 @@ nce_stats_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_co
                 tma_load_2d(cl, full_bar, smem + 3 * kTileABytes, kx, jt * kNceTile, kEvictLast);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            for (int kb = 0; kb < nkb; ++kb) {
-                mbar_wait(full_bar, (uint32_t)kb & 1u);
-                tc_fence_after();
-                const uint32_t t0 = smem_u32(smem);
-#pragma unroll
-                for (int k = 0; k < kBlockK / 16; ++k) {
-                    const uint32_t off = k * 32;
-                    uint64_t dsc[4];
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) dsc[q] = make_sw128_kmajor_desc(t0 + q * kTileABytes + off);
-                    const uint32_t acc = (kb > 0 || k > 0) ? 1u : 0u;
-                    umma_bf16(tmem_base, dsc[0], dsc[2], kNceIdesc, acc);      // hi hi + hi lo + lo hi
-                    umma_bf16(tmem_base, dsc[0], dsc[3], kNceIdesc, 1u);
-                    umma_bf16(tmem_base, dsc[1], dsc[2], kNceIdesc, 1u);
-                }
-                umma_commit(empty_bar);
-            }
-            umma_commit(accum_bar);
-        }
     } else {
-        // 8 epilogue warps: lane quarter q = warp & 3 (the TMEM lanes a warp may read), column half h of every accumulator
-        const int q = warp & 3, h = (warp - 2) >> 2;
-        const int64_t i = (int64_t)it * kNceTile + q * 32 + lane;
-        const int64_t j0 = (int64_t)jt * kNceTile;
-        const int64_t ntj = 2 * (int64_t)gridDim.y;                   // row-sum partials: one per (column tile, half)
-        const float scale = inv_tau * 1.4426950408889634f;          // exp(x) = exp2(x log2 e)
-        mbar_wait(accum_bar, 0);
-        tc_fence_after();
-        // A warp owns 32 rows x 64 columns of every accumulator.  Its exponentials go to global memory through a shared-memory
-        // staging tile (row stride 144 B: conflict-free 128-bit accesses both ways) so that 8 lanes write one 128-byte row
-        // segment: 4 cache lines per store instruction instead of 32 (the thread-per-row stores cost 12 us, round 2 trace).
-        uint8_t* stage_hi = smem + (warp - 2) * (2 * kNceRows * kNceRowPitch);
-        uint8_t* stage_lo = stage_hi + kNceRows * kNceRowPitch;
-        const int c0 = h * (kNceTile / 2);
-        const bool plain = (int64_t)(it + 1) * kNceTile <= n && (int64_t)(jt + 1) * kNceTile <= n && it != jt;   // CTA-uniform
-        {
-            float part = 0.f;
 #pragma unroll
-            for (int cc = 0; cc < kNceTile / 2; cc += 32) {
-                const int c = c0 + cc;
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-                uint32_t ph[16], pl[16];
-                // interior tiles off the diagonal (most of them) skip the bounds and diagonal tests: 6 instead of 11 instructions
-                // per exponential
-                if (plain) part += nce_exp32<false>(v, scale, i, j0 + c, n, nullptr, ph, pl);
-                else part += nce_exp32<true>(v, scale, i, j0 + c, n, mat < 2 ? stats + mat * n : nullptr, ph, pl);
+        for (int j = 0; j < kNceTile / 2; ++j) acc[j] = 0.f;
+        mma_kblocks<kNceTile, 1, kNceStageBytes>(acc, smem, full_bar, empty_bar, 0, nkb);     // hi hi + hi lo + lo hi
+    }
+    __syncthreads();            // every MMA has read the operand tiles: the staging area may overwrite them
+    if (warp == kProducerWarp) return;
+
+    // A warp owns 16 rows x 128 columns of the tile (rows r and r + 8 per lane, wgmma fragment layout).  Exponentials, their row
+    // sums per column half (the two partials of this column tile in the stats layout) and the diagonal; the exponentials go to
+    // global memory as bf16 hi / lo through a shared-memory staging tile (row pitch 272 B: conflict-free both ways) so that
+    // 16 lanes write one 256-byte row segment.
+    const int64_t rbase = (int64_t)it * kNceTile + 64 * (warp >> 2) + 16 * (warp & 3);
+    const int64_t j0 = (int64_t)jt * kNceTile;
+    const int64_t ntj = 2 * (int64_t)gridDim.y;                   // row-sum partials: one per (column tile, half)
+    const float scale = inv_tau * 1.4426950408889634f;          // exp(x) = exp2(x log2 e)
+    const bool plain = (int64_t)(it + 1) * kNceTile <= n && (int64_t)(jt + 1) * kNceTile <= n && it != jt;   // CTA-uniform
+    float* diag = mat < 2 ? stats + mat * n : nullptr;
+    uint8_t* stage_hi = smem + warp * (2 * kNceRows * kNceRowPitch);
+    uint8_t* stage_lo = stage_hi + kNceRows * kNceRowPitch;
+    float part[2][2] = {{0.f, 0.f}, {0.f, 0.f}};                  // [row r / r + 8][column half]
 #pragma unroll
-                for (int t = 0; t < 16; t += 4) {
-                    *reinterpret_cast<uint4*>(stage_hi + lane * kNceRowPitch + cc * 2 + t * 4) = make_uint4(ph[t], ph[t + 1], ph[t + 2], ph[t + 3]);
-                    *reinterpret_cast<uint4*>(stage_lo + lane * kNceRowPitch + cc * 2 + t * 4) = make_uint4(pl[t], pl[t + 1], pl[t + 2], pl[t + 3]);
-                }
+    for (int j = 0; j < kNceTile / 2; j += 2) {
+        const int rr = (j >> 1) & 1, h = j >= kNceTile / 4 ? 1 : 0;
+        const int rl = (lane >> 2) + 8 * rr, cl = frag_col(lane, j);
+        const int64_t i = rbase + rl, col = j0 + cl;
+        float e0, e1;
+        if (plain) {            // interior tiles off the diagonal (most of them) skip the bounds and diagonal tests
+            e0 = fast_exp2(acc[j] * scale);
+            e1 = fast_exp2(acc[j + 1] * scale);
+        } else {
+            e0 = (i < n && col < n) ? fast_exp2(acc[j] * scale) : 0.f;
+            e1 = (i < n && col + 1 < n) ? fast_exp2(acc[j + 1] * scale) : 0.f;
+            if (diag != nullptr && i < n) {
+                if (i == col) diag[i] = e0;
+                if (i == col + 1) diag[i] = e1;
             }
-            __syncwarp();
-            // rows up to the padded height are written (zeros beyond n): the backward's GEMMs read them as K padding
-            const int64_t row_base = (int64_t)it * kNceTile + q * 32;
-            uint16_t* ghi = e_hi + (int64_t)mat * lde * lde + row_base * lde + j0 + c0;
-            uint16_t* glo = e_lo + (int64_t)mat * lde * lde + row_base * lde + j0 + c0;
+        }
+        part[rr][h] += e0 + e1;
+        const uint32_t hp = pack_bf16(e0, e1);
+        *reinterpret_cast<uint32_t*>(stage_hi + rl * kNceRowPitch + cl * 2) = hp;
+        *reinterpret_cast<uint32_t*>(stage_lo + rl * kNceRowPitch + cl * 2) =
+            pack_bf16(e0 - __uint_as_float(hp << 16), e1 - __uint_as_float(hp & 0xffff0000u));
+    }
 #pragma unroll
-            for (int r0 = 0; r0 < kNceRows; r0 += 4) {
-                const int r = r0 + (lane >> 3), ch = lane & 7;
-                *reinterpret_cast<uint4*>(ghi + (int64_t)r * lde + ch * 8) = *reinterpret_cast<const uint4*>(stage_hi + r * kNceRowPitch + ch * 16);
-                *reinterpret_cast<uint4*>(glo + (int64_t)r * lde + ch * 8) = *reinterpret_cast<const uint4*>(stage_lo + r * kNceRowPitch + ch * 16);
+    for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) part[rr][h] = group_sum<4>(part[rr][h], group_mask<4>());
+    if (mat < 2 && (lane & 3) == 0) {
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+            const int64_t i = rbase + (lane >> 2) + 8 * rr;
+            if (i < n) {
+                stats[4 * n + mat * ntj * n + (2 * jt) * n + i] = part[rr][0];
+                stats[4 * n + mat * ntj * n + (2 * jt + 1) * n + i] = part[rr][1];
             }
-            if (i < n && mat < 2) stats[4 * n + mat * ntj * n + (2 * jt + h) * n + i] = part;
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(128) : "memory");
+    __syncwarp();
+    // rows up to the padded height are written (zeros beyond n): the backward's GEMMs read them as K padding
+    uint16_t* ghi = e_hi + (int64_t)mat * lde * lde + rbase * lde + j0;
+    uint16_t* glo = e_lo + (int64_t)mat * lde * lde + rbase * lde + j0;
+#pragma unroll
+    for (int r0 = 0; r0 < kNceRows; r0 += 2) {
+        const int r = r0 + (lane >> 4), ch = lane & 15;
+        *reinterpret_cast<uint4*>(ghi + (int64_t)r * lde + ch * 8) = *reinterpret_cast<const uint4*>(stage_hi + r * kNceRowPitch + ch * 16);
+        *reinterpret_cast<uint4*>(glo + (int64_t)r * lde + ch * 8) = *reinterpret_cast<const uint4*>(stage_lo + r * kNceRowPitch + ch * 16);
     }
 }
 

@@ -1,5 +1,5 @@
 // Helpers around the projection GEMMs (nn.Linear image_trans / text_trans, Models.py:28-31,173-174):
-//  * fp32 -> (bf16 hi, bf16 lo) operand split (x ~= hi + lo with ~16 mantissa bits) so the tcgen05
+//  * fp32 -> (bf16 hi, bf16 lo) operand split (x ~= hi + lo with ~16 mantissa bits) so the wgmma
 //    kernel can reach fp32-level accuracy with three bf16 MMAs per product;
 //  * split-K reduction epilogues: bias + dropout mask for the forward, transpose for the weight grad.
 #include <cuda_bf16.h>

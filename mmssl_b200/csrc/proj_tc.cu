@@ -1,10 +1,10 @@
-// Projection GEMM on the 5th-gen tensor cores (tcgen05) fed by TMA, accumulators in TMEM.
+// Projection GEMM on the Hopper tensor cores (wgmma) fed by TMA, accumulators in registers.
 //
 //   partial[s][m][n] = sum_{k in slice s} (A_hi + A_lo)[m][k] * (B_hi + B_lo)[n][k]      (lo*lo dropped)
 //
 // replaces nn.Linear image_trans / text_trans forward (X = F W^T, Models.py:173-174) and its weight
 // gradient (dW^T = F^T dX, autograd of the same lines).  fp32 contract (1e-4 rel) is met with a
-// bf16 hi/lo operand split: three kind::f16 MMAs per product, fp32 accumulation in TMEM.  The
+// bf16 hi/lo operand split: three bf16 MMAs per product, fp32 accumulation in registers.  The
 // feature matrix is constant (Models.py:46-47), so its split (and its transposed split for the
 // weight gradient) is made once; both GEMMs then run the SAME K-major kernel.
 //
@@ -12,10 +12,10 @@
 // medium (feature dim) -> split-K so that >= 2 waves of CTAs pull from HBM; partials are reduced in
 // a fixed order by the epilogue kernels in proj_common.cu (deterministic, no float atomics).
 //
-// Kernel anatomy (one CTA = one 128 x N output tile of one K slice, 192 threads):
-//   warp 0  : TMA producer   (cp.async.bulk.tensor.2d, SWIZZLE_128B, mbarrier complete_tx)
-//   warp 1  : TMEM alloc + single-thread tcgen05.mma issuer, tcgen05.commit frees smem stages
-//   warps 2-5: epilogue       (tcgen05.ld 32x32b -> registers -> 128-bit global stores)
+// Kernel anatomy (one CTA = one 128 x N output tile of one K slice, 288 threads, tc_common.cuh):
+//   warps 0-7: two consumer warpgroups, 64 rows each: wgmma.mma_async m64nNk16 from the swizzled smem tiles, each warp
+//              releases a stage once its MMAs have completed; epilogue straight from the accumulator registers
+//   warp 8   : TMA producer (cp.async.bulk.tensor.2d, SWIZZLE_128B, mbarrier complete_tx)
 #include "tc_common.cuh"
 #include "../../include/mmssl_b200.h"
 
@@ -30,8 +30,6 @@ struct GemmCfg {
     static constexpr int kCtasPerSm = (N == 64) ? 2 : 1;
     static constexpr int kStages = (N == 64) ? 2 : (N == 128 ? 3 : 2);
     static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-    static constexpr uint32_t kIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) |
-                                       ((uint32_t)(kBlockM >> 4) << 24);   // F32 acc, BF16 x BF16, K-major both
 };
 
 template <int N>
@@ -44,36 +42,23 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_con
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
     uint64_t* empty_bar = full_bar + Cfg::kStages;
-    uint64_t* accum_bar = empty_bar + Cfg::kStages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m_tile = blockIdx.x, split = blockIdx.y;
     const int kb0 = split * kb_per_split;
     const int nkb = max(0, min(total_kb, kb0 + kb_per_split) - kb0);
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_a_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_a_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tm_b_lo) : "memory");
+        for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-            mbar_init(accum_bar, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(N) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         if (lane == 0) {
             for (int i = 0; i < nkb; ++i) {
                 const int s = i % Cfg::kStages;
@@ -88,70 +73,31 @@ gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_con
                 tma_load_2d(&tm_b_lo, &full_bar[s], st + 2 * kTileABytes + Cfg::kTileBBytes, kx, 0, kEvictLast);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            for (int i = 0; i < nkb; ++i) {
-                const int s = i % Cfg::kStages;
-                const uint32_t ph = (uint32_t)(i / Cfg::kStages) & 1u;
-                mbar_wait(&full_bar[s], ph);
-                tc_fence_after();
-                const uint32_t a_hi = smem_u32(smem + s * Cfg::kStageBytes);
-                const uint32_t a_lo = a_hi + kTileABytes;
-                const uint32_t b_hi = a_hi + 2 * kTileABytes;
-                const uint32_t b_lo = b_hi + Cfg::kTileBBytes;
-#pragma unroll
-                for (int k = 0; k < kBlockK / 16; ++k) {
-                    const uint32_t off = k * 32;   // 16 bf16 = 32 bytes inside the 128-byte swizzle span
-                    const uint64_t dah = make_sw128_kmajor_desc(a_hi + off), dal = make_sw128_kmajor_desc(a_lo + off);
-                    const uint64_t dbh = make_sw128_kmajor_desc(b_hi + off), dbl = make_sw128_kmajor_desc(b_lo + off);
-                    umma_bf16(tmem_base, dah, dbh, Cfg::kIdesc, (i > 0 || k > 0) ? 1u : 0u);
-                    umma_bf16(tmem_base, dah, dbl, Cfg::kIdesc, 1u);
-                    umma_bf16(tmem_base, dal, dbh, Cfg::kIdesc, 1u);
-                }
-                umma_commit(&empty_bar[s]);   // frees the smem stage once the MMAs have read it
-            }
-            umma_commit(accum_bar);           // accumulator complete
-        }
     } else {
-        const int q = warp & 3;               // TMEM lane quarter this warp may access
-        const int64_t row = (int64_t)m_tile * kBlockM + q * 32 + lane;
-        float* out = partial + ((int64_t)split * M + row) * N;
-        if (nkb > 0) {
-            mbar_wait(accum_bar, 0);
-            tc_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < N; c += 32) {
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c, v);
-                if (row < M) {
+        float acc[N / 2];
 #pragma unroll
-                    for (int j = 0; j < 32; j += 4)
-                        st4(out + c + j, make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                     __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3])));
-                }
-            }
-        } else if (row < M) {
-            for (int c = 0; c < N; c += 4) st4(out + c, f4zero());
+        for (int j = 0; j < N / 2; ++j) acc[j] = 0.f;
+        mma_kblocks<N, Cfg::kStages, Cfg::kStageBytes>(acc, smem, full_bar, empty_bar, 0, nkb);
+        const int64_t row0 = (int64_t)m_tile * kBlockM + 64 * (warp >> 2);
+        float* out = partial + ((int64_t)split * M) * N;
+#pragma unroll
+        for (int j = 0; j < N / 2; j += 2) {
+            const int64_t row = row0 + frag_row(warp, lane, j);
+            if (row < M) *reinterpret_cast<float2*>(out + row * N + frag_col(lane, j)) = make_float2(acc[j], acc[j + 1]);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(N) : "memory");
     }
 }
 
 static int choose_split(int64_t m, int64_t n, int64_t k) {
     // HBM-bound streaming GEMM: what matters is that all SMs pull from HBM for the whole kernel.
     // Pick the split-K that fills ONE wave of co-resident CTAs as completely as possible
-    // (e.g. 56 M-tiles x 5 slices = 280 of 296 slots) instead of leaving a nearly empty tail wave.
+    // (e.g. 56 M-tiles x 4 slices = 224 of 264 slots) instead of leaving a nearly empty tail wave.
     const int64_t total_kb = (k + kBlockK - 1) / kBlockK;
     const int64_t m_tiles = (m + kBlockM - 1) / kBlockM;
     const int64_t slots = (int64_t)kNumSMs * (n == 64 ? 2 : 1);
     int64_t split = slots / m_tiles;
     // accuracy: the tensor core's fp32 accumulate is not round-to-nearest and its error grows linearly with the number of MMAs
-    // chained into one TMEM accumulator (gemm_wide.cu; measured round 2: the weight gradient at 200k items, 347 k-blocks per
-    // slice, was 1e-4 off).  A slice is therefore at most kMaxChainKb k-blocks long; the slices are summed in fp32 by the epilogue.
+    // chained into one accumulator (gemm_wide.cu; the weight gradient at 200k items with 347 k-blocks per slice was 1e-4 off).  A slice is therefore at most kMaxChainKb k-blocks long; the slices are summed in fp32 by the epilogue.
     const int64_t need = (total_kb + kMaxChainKb - 1) / kMaxChainKb;
     if (split < need) split = need;
     if (split > kMaxSplit) split = kMaxSplit;

@@ -1,5 +1,5 @@
 // CUDA-core fp32 GEMM (64x64x16 tiles, 4x4 per thread).  Not the projection's production path
-// (that is the tcgen05 kernel in proj_tc.cu); used for the small d x d mixing GEMMs of the
+// (that is the wgmma kernel in proj_tc.cu); used for the small d x d mixing GEMMs of the
 // "attention" closed form (Models.py:139-169, SURVEY appendix B.1), their gradients, and as the
 // independent verification path for the tensor-core projection.
 #include "common.cuh"

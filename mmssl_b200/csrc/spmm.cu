@@ -2,7 +2,7 @@
 // path (reference: MMSSL.mm / torch.sparse.mm, Models.py:69-73, and torch.mm(sparse, dense),
 // Models.py:203-208; the transposed products autograd derives from them use the CSR of A^T).
 //
-// B200 design (sparse gather: latency bound on small graphs, L2-gather / resident-row-walk bound on
+// Design (sparse gather: latency bound on small graphs, L2-gather / resident-row-walk bound on
 // large ones -- DESIGN.md section 6; no tensor cores):
 //  * one lane *group* (16 lanes for d=64, 32 lanes for d>=128) owns one work item = one row or one
 //    fixed-length segment of a long row (plan built by mmssl_spmm_plan); every lane owns one
@@ -36,8 +36,8 @@ namespace mmssl {
 // output, the running-sum base -- are requested as soon as the work item is known, so that they travel while the
 // index -> gather chain runs instead of adding one more dependent round trip after it.  Only for R*C <= 2 (register cost).
 // HINT (large graphs, impl bits 7 / 8): 1 = the streams (col, val, outputs, row-indexed operands) are marked L2 evict-first and
-// bypass L1 so that they do not push the gathered table out of L2 (measured round 1: DRAM traffic 2.18x the compulsory bytes
-// at 1M x 200k because a 102 MB table shares the L2 with 670 MB of streams); 2 = additionally the column indices carry a
+// bypass L1 so that they do not push the gathered table out of L2 (at 1M x 200k a 102 MB table shares the L2 with 670 MB of
+// streams, so the gathered rows are re-fetched from DRAM); 2 = additionally the column indices carry a
 // "hot" flag in the sign bit (the head of the column-degree distribution, graph.py:hot_flag_plan) and hot rows are loaded
 // with L1::evict_last, cold ones with L1::no_allocate, so that the ~200 KB of L1 serve the popular rows.
 // One work item, from its descriptor and the first chunk of (col, val) pairs (one per lane, 0 beyond the item's end) to the
@@ -293,8 +293,7 @@ __global__ void __launch_bounds__(256, MINB) spmm_csr_kernel(const SpmmParams p)
 // items gid, gid + stride, ... .  While item k is gathered, the (col, val) chunk of item k+1 and the descriptor of item k+2 are
 // already in flight (and, PRE, the row-indexed epilogue operands of item k are requested before its gathers), so that an item
 // costs about one memory round trip (its gathers) instead of the four of the one-item kernel (descriptor -> indices ->
-// gathers -> epilogue operands), and a plan of 2.4 waves no longer pays them per wave (ncu, round 2: 66 registers -> 7 blocks
-// per SM -> 2452 blocks = 2.37 waves, SMs 62 % active).  Per-item arithmetic is spmm_item's: results are identical.
+// gathers -> epilogue operands), and a plan of several waves no longer pays them per wave.  Per-item arithmetic is spmm_item's: results are identical.
 template <int G, int C, int R, bool PRE>
 __global__ void __launch_bounds__(128) spmm_csr_pipe_kernel(const SpmmParams p) {
     pdl_wait();

@@ -4,7 +4,7 @@
 // memory; only cold neighbours go through the L2 gather path.
 //
 // Why: at 1M x 200k / 20M edges the LDG kernel (spmm.cu) is bound by the L2 -> SM gather stream
-// (each of the nnz neighbour rows crosses L2 once: 4*d*nnz bytes, ~9 TB/s), not by HBM.  With
+// (each of the nnz neighbour rows crosses L2 once: 4*d*nnz bytes), not by HBM.  With
 // Zipf-like item popularity a few hundred columns carry about half of the edges, and ~200 KB of
 // shared memory holds 400 (d=128) .. 800 (d=64) rows, so about half of that stream disappears.
 //

@@ -387,8 +387,8 @@ class Engine:
                 return oa, (oa if same else ob), part
 
             # The user-side fusion backward needs only g_eu = inv * g_uf, not the chain: it runs beside the chain on the pair
-            # stream (after the chain it had to share the SMs with the weight-gradient GEMMs' 200 KB CTAs: 36 us instead of 10,
-            # round-2 trace); only the item side, which reads the chain's result g_ei, follows the chain.
+            # stream (after the chain it had to share the SMs with the weight-gradient GEMMs' large CTAs and ran several times
+            # slower on the earlier hardware); only the item side, which reads the chain's result g_ei, follows the chain.
             def user_side():
                 ops.axpby(g_uf, inv, 0.0, g_eu)
                 return fuse_bwd2(g_eu, st.zn_u, st.nrm_u, uvid, utid, g_uvid, g_utid)

@@ -248,7 +248,7 @@ class FullStep:
         """Capture one steady-state iteration (D step + G step + both optimisers, ~150 launches) into a CUDA graph; ``step``
         replays it whenever ``steady()`` holds and runs eagerly otherwise (first iterations of an epoch).  The random draws
         are static input buffers refilled before every replay (by torch's generator, or by the caller's injected draws).
-        Green on hardware since round 2 (tests/test_gpu_zzz_gemm_wide.py::test_full_step_cuda_graph_replay_equals_eager).
+        Green on the H100 (tests/test_gpu_zzz_gemm_wide.py::test_full_step_cuda_graph_replay_equals_eager).
         NOTE: the warm-up below is ONE REAL iteration on the indices currently in ``hs.idx`` with draws from torch's generator
         (both optimisers step, BatchNorm statistics move): call it where an iteration of the run belongs (trainer.py does), not
         in front of one."""

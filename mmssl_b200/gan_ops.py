@@ -1,11 +1,11 @@
 """CUDA backend of the GAN-side ops (csrc/gan.cu) -- the namespace ``mmssl_b200.gan`` is given as ``K`` in the product.
 One function per op of tests/gan_ops_cpu.py (its specification), same names and argument meaning; outputs are allocated
 here, every call goes through the C ABI and raises when the extension or a CUDA device is missing (no CPU fallback).
-GEMMs: ``GEMM_IMPL = "tc"`` routes every product through the general-width tcgen05 kernel (csrc/gemm_wide.cu; operands
+GEMMs: ``GEMM_IMPL = "tc"`` routes every product through the general-width wgmma kernel (csrc/gemm_wide.cu; operands
 split into bf16 hi/lo pairs, K-major, by the same split kernels as the projection); ``"simt"`` is the fp32 CUDA-core GEMM.
-"tc" is the default since round 2: gemm_wide.cu is parity-green on B200 (tests/test_gpu_zzz_gemm_wide.py; its accumulation
-passes are bounded, error 6e-6 max-norm at K = 7050 against 3.9e-6 for fp32 cuBLAS) and the full iteration on it is 9.1 ms at
-Baby against 22.2 ms on the CUDA-core route (tools/fullstep_bench.py); ``MMSSL_GAN_GEMM=simt`` or ``gan_ops.GEMM_IMPL`` switch.  ``"cublas"`` sends the same products to the vendor library through
+"tc" is the default: gemm_wide.cu is parity-green on the H100 (tests/test_gpu_zzz_gemm_wide.py; its accumulation
+passes are bounded) and the full iteration on it is about 3x faster than on the CUDA-core route at Baby (tools/fullstep_bench.py;
+the H100 numbers are in DESIGN section 6); ``MMSSL_GAN_GEMM=simt`` or ``gan_ops.GEMM_IMPL`` switch.  ``"cublas"`` sends the same products to the vendor library through
 ``torch.mm`` / ``addmm`` (fp32, TF32 off): the library baseline the tensor-core kernel is measured against
 (tools/fullstep_bench.py --gemm cublas), not the product path."""
 from __future__ import annotations

@@ -285,7 +285,7 @@ def infonce_forward(z1, z2, idx, inv_tau: float, work: InfoNCEWork, g_loss=None)
     """prepare + stats: fills work.loss_part (sum = n * loss) and the backward coefficients."""
     lib = _lib_()
     n, d = work.n, work.d
-    if work.tc:      # gather + normalise + bf16 hi/lo split in one kernel, similarity tiles on tcgen05, finalize
+    if work.tc:      # gather + normalise + bf16 hi/lo split in one kernel, similarity tiles on wgmma, finalize
         _lib.check(lib.mmssl_infonce_forward_tc(ptr(z1), _ld(z1), ptr(z2), _ld(z2), ptr(idx), n, d, float(inv_tau), ptr(work.a), ptr(work.b),
                                                 ptr(work.na), ptr(work.nb), ptr(work.stats), ptr(work.coef), ptr(g_loss),
                                                 ptr(work.loss_part), ptr(work.ws), work.ws.numel(), stream()))
@@ -406,7 +406,7 @@ def split_bf16_t(x, mask=None, ldo=None, out=None, colsum=None):
 
 
 def gemm_bf16x3_wide(a_hi, a_lo, b_hi, b_lo, m, n, k, out, alpha: float = 1.0, accumulate: bool = False):
-    """out[m, n] (+)= alpha * (a_hi + a_lo)[m,k] @ (b_hi + b_lo)[n,k]^T on tcgen05 tensor cores, any n (csrc/gemm_wide.cu)."""
+    """out[m, n] (+)= alpha * (a_hi + a_lo)[m,k] @ (b_hi + b_lo)[n,k]^T on wgmma tensor cores, any n (csrc/gemm_wide.cu)."""
     lib = _lib_()
     assert out.dtype == torch.float32 and out.stride(1) == 1 and out.shape == (m, n)
     _lib.check(lib.mmssl_gemm_bf16x3_wide(ptr(a_hi), ptr(a_lo), a_hi.stride(0), ptr(b_hi), ptr(b_lo), b_hi.stride(0), m, n, k,
@@ -415,7 +415,7 @@ def gemm_bf16x3_wide(a_hi, a_lo, b_hi, b_lo, m, n, k, out, alpha: float = 1.0, a
 
 
 def gemm_wide_set_chunk(k_blocks: int) -> None:
-    """k-blocks (64 of K) accumulated in TMEM before a pass is folded into C in fp32 (default 16; csrc/gemm_wide.cu)."""
+    """k-blocks (64 of K) accumulated in registers before a pass is folded into C in fp32 (default 16; csrc/gemm_wide.cu)."""
     _lib.check(_lib_().mmssl_gemm_wide_set_chunk(int(k_blocks)))
 
 
@@ -437,7 +437,7 @@ def gemm_bf16x3_plan(m, n, k):
 
 
 def gemm_bf16x3(a_hi, a_lo, b_hi, b_lo, m, n, k, split_k, partial):
-    """partial[s][m][n] = K-slice s of (a_hi + a_lo)[m,k] @ (b_hi + b_lo)[n,k]^T on tcgen05 tensor cores."""
+    """partial[s][m][n] = K-slice s of (a_hi + a_lo)[m,k] @ (b_hi + b_lo)[n,k]^T on wgmma tensor cores."""
     lib = _lib_()
     _lib.check(lib.mmssl_gemm_bf16x3(ptr(a_hi), ptr(a_lo), a_hi.stride(0), ptr(b_hi), ptr(b_lo), b_hi.stride(0), m, n, k,
                                      split_k, ptr(partial), stream()))

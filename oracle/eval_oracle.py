@@ -3,7 +3,7 @@
 Only ``tests/`` may import this module; nothing under ``mmssl_b200/`` does.
 
 Restates in numpy what the reference computes in ``Trainer.test`` (citations relative to
-/root/reference/MMSSL/):
+MMSSL/ of the reference repository):
 
   * dense scoring of a user batch against all items            utility/batch_test.py:147-154
   * per user: drop the training items, take the max(Ks) best   utility/batch_test.py:21-36, :83-107

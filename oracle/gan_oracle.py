@@ -2,7 +2,7 @@
 (D step + G step) it is part of.  TEST INFRASTRUCTURE -- NOT PRODUCT CODE; only ``tests/`` may import it.
 
 Restated on stock CPU torch, gradients by torch autograd -- the engine the reference itself uses (citations relative to
-/root/reference/MMSSL/):
+MMSSL/ of the reference repository):
 
   * u_sim_calculation            main.py:283-298   dense [B, I] scores, training items zeroed, rows L2-normalised
   * Discriminator                Models.py:224-245 Linear -> LeakyReLU(True) -> BatchNorm1d -> Dropout, twice, Linear -> Sigmoid, x100

@@ -4,7 +4,7 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline``
 ``--impl reference`` legs may import this module.  Nothing under ``mmssl_b200/`` does.
 
 It restates, op by op and on stock CPU torch, the algorithm of the reference's per-step hot
-path (citations are relative to /root/reference/MMSSL/):
+path (citations are relative to MMSSL/ of the reference repository):
 
   * graph normalisation            main.py:89-112, :513-520
   * MMSSL.forward                  Models.py:139-220

@@ -9,13 +9,13 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu through gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
 
 
 def pytest_addoption(parser):
     parser.addoption("--cuemu", action="store_true", default=False,
                      help="run the tests marked `gpu` on the CPU under the cuemu fiber emulator (tests/cuemu): "
-                          "`pytest tests -m gpu --cuemu`.  Tests that need TMA / tcgen05 / multimem PTX, CUDA graphs or 2 GPUs fail or skip.")
+                          "`pytest tests -m gpu --cuemu`.  Tests that need CUDA graphs or 2 GPUs fail or skip.")
 
 
 import pytest  # noqa: E402

@@ -5,7 +5,7 @@ The sources are mmssl_b200/csrc/*.cu, untouched except for three pieces of synta
   kernel<<<grid, block, smem, stream>>>(args)   ->  cuemu::launch(kernel, cuemu::cfg(grid, block, smem, stream), "kernel")(args)
   extern __shared__ [__align__(n)] T name[];    ->  T* name = (T*)cuemu::dyn_smem();
   asm volatile("ptx" : outs : ins : ...);       ->  cuemu::ptx_op("ptx", &outs, sizes, n, ins, n)   (cuemu_ptx.cpp: a functional model of
-                                                    the mbarrier / TMA / tcgen05 subset the library uses; anything else fails the launch)
+                                                    the mbarrier / TMA / wgmma subset the library uses; anything else fails the launch)
 CUB's SortPairs / ExclusiveSum are host shims (include/cub/cub.cuh).  Every .cu of the library is compiled.
 
     python -m tests.cuemu.build [--force]
@@ -72,7 +72,7 @@ _STRLIT = re.compile(r'"((?:[^"\\]|\\.)*)"')
 def _strip_asm(src: str) -> str:
     """asm volatile("template" : outputs : inputs : clobbers);  ->  a call of cuemu::ptx_op with the template text, pointers to
     the output operands and the input operands as 64-bit values (floats by bit pattern).  include/cuemu_ptx.h interprets the
-    subset of PTX the library uses (mbarrier, TMA tensor copies, tcgen05, griddepcontrol) and fails the launch on the rest."""
+    subset of PTX the library uses (mbarrier, TMA tensor copies, wgmma, griddepcontrol) and fails the launch on the rest."""
     out, pos = [], 0
     while True:
         m = _ASM.search(src, pos)

@@ -1,22 +1,22 @@
 // cuemu: functional model of the inline PTX the library uses.  TEST INFRASTRUCTURE ONLY (see include/cuemu.h).
 //
-// Scope = exactly what csrc/tc_common.cuh, proj_tc.cu and gemm_wide.cu issue:
+// Scope = exactly what csrc/tc_common.cuh and the kernels built on it issue:
 //   mbarrier.init / arrive / arrive.expect_tx / try_wait.parity         phase + pending-arrival + transaction-byte counters
 //   cp.async.bulk (1-D) ... mbarrier::complete_tx::bytes       contiguous copy global -> shared (spmm_hot.cu)
 //   cp.async.bulk.tensor.2d ... mbarrier::complete_tx::bytes    box copy global -> shared through the tensor map: out-of-bounds
 //                                                               elements read as zero, SWIZZLE_128B (address bits [4:6] ^= [7:9])
-//   tcgen05.alloc / dealloc / relinquish_alloc_permit           a 128-lane x 512-column fp32 TMEM per block
-//   tcgen05.mma.cta_group::1.kind::f16                          D[128 x N] (+)= A[128 x 16] * B[N x 16]^T, bf16 operands read from
-//                                                               shared memory through K-major SWIZZLE_128B descriptors
-//   tcgen05.commit ... mbarrier::arrive::one                    (the model executes an MMA when it is issued, so commit = arrive)
-//   tcgen05.ld.sync.aligned.32x32b.x32                          lane t of warp w reads TMEM lane 32*(w%4)+t, 32 columns
+//   wgmma.mma_async.sync.aligned.m64nNk16.f32.bf16.bf16         D[64 x N] += A[64 x 16] * B[N x 16]^T, bf16 operands read from
+//                                                               shared memory through K-major SWIZZLE_128B descriptors; each
+//                                                               thread updates its own accumulator fragment when it issues the
+//                                                               instruction (the model executes an MMA at once)
+//   wgmma.fence / commit_group / wait_group                     no-ops (the MMA has already executed)
 //   multimem.ld_reduce.add.v4.f32 / multimem.st.v4.f32         over multicast groups registered by the test (cuemu_mc_register):
 //                                                               several ranks' replicas in one process
-//   fences, prefetch.tensormap, tcgen05.wait::ld, griddepcontrol.wait   no-ops
-// What the model asserts on the way: 1024-byte aligned swizzled tiles, transaction bytes that add up, barrier phases, a warp
-// touching only its TMEM lane quarter, descriptor fields the kernels are supposed to encode.  It is calibrated by running
-// proj_tc.cu -- which is parity-green on real B200s -- through it (tests/test_emu_tensor_core.py): a kernel that passes here
-// and shares tc_common.cuh's descriptor / swizzle code with it differs from hardware-proven code only in its own logic.
+//   fences, prefetch.tensormap, griddepcontrol.wait             no-ops
+// What the model asserts on the way: 1024-byte aligned swizzled tiles, transaction bytes that add up, barrier phases, the
+// descriptor fields the kernels are supposed to encode, the accumulator fragment size of the instruction shape.  A kernel that
+// passes here and shares tc_common.cuh's descriptor / swizzle code with proj_tc.cu (tests/test_emu_tensor_core.py) differs
+// from the kernel the GPU tests check only in its own logic.
 // It says nothing about timing, asynchrony bugs that need real concurrency, or PTX outside this list (fails the launch).
 #include <map>
 #include <string>
@@ -58,9 +58,6 @@ const McGroup& mc_find(uint64_t addr, size_t bytes, uint64_t* off) {
     *off = 0;
     return none;
 }
-std::vector<uint32_t> g_tmem;              // [128 lanes][512 columns]
-int g_tmem_cols = 0;
-
 uint8_t* smem_at(uint64_t addr, size_t bytes) {
     if (addr + bytes > dyn_smem_bytes()) fail("shared-memory address outside the block's dynamic shared memory");
     return static_cast<uint8_t*>(dyn_smem()) + addr;
@@ -118,14 +115,12 @@ CUresult encode_tiled(CUtensorMap* map, CUtensorMapDataType dt, cuuint32_t rank,
 
 void ptx_block_reset() {
     g_bars.clear();
-    g_tmem.assign(128 * 512, 0x7FC00000u);      // NaN until written
-    g_tmem_cols = 0;
 }
 
 void ptx_op(const char* text, void** outs, const int* out_sizes, int n_out, const uint64_t* in, int n_in) {
     auto has = [&](const char* s) { return strstr(text, s) != nullptr; };
-    if (has("griddepcontrol") || has("tcgen05.fence") || has("fence.mbarrier_init") || has("prefetch.tensormap") ||
-        has("tcgen05.wait::ld") || has("tcgen05.relinquish_alloc_permit"))
+    if (has("griddepcontrol") || has("fence.mbarrier_init") || has("prefetch.tensormap") || has("wgmma.fence") ||
+        has("wgmma.commit_group") || has("wgmma.wait_group"))
         return;
     if (has("ex2.approx")) {                                  // MUFU.EX2: the model returns the correctly rounded value
         float x;
@@ -214,81 +209,41 @@ void ptx_op(const char* text, void** outs, const int* out_sizes, int n_out, cons
         bar_check(b);
         return;
     }
-    if (has("tcgen05.alloc")) {
-        if (cur->lane != 0) return;               // .sync.aligned: one allocation per warp, every lane executes the instruction
-        const int ncols = (int)in[1];
-        if (ncols < 32 || ncols > 512 || (ncols & (ncols - 1))) fail("tcgen05.alloc: column count must be a power of two in [32, 512]");
-        if (g_tmem_cols + ncols > 512) fail("tcgen05.alloc: TMEM exhausted");
-        const uint32_t base = (uint32_t)g_tmem_cols;              // lane 0, first free column
-        g_tmem_cols += ncols;
-        memcpy(smem_at(in[0], 4), &base, 4);
-        return;
-    }
-    if (has("tcgen05.dealloc")) {
-        if (cur->lane != 0) return;
-        g_tmem_cols -= (int)in[1];
-        if (g_tmem_cols < 0) fail("tcgen05.dealloc of more columns than allocated");
-        return;
-    }
-    if (has("tcgen05.mma")) {
-        if (!has("kind::f16") || !has("cta_group::1")) fail("tcgen05.mma: only cta_group::1.kind::f16 is modelled");
-        const uint32_t tm = (uint32_t)in[0], idesc = (uint32_t)in[3];
-        const uint64_t da = in[1], db = in[2];
-        const bool acc = in[4] != 0;
-        const int N = (int)((idesc >> 17) & 0x3Fu) << 3, M = (int)((idesc >> 24) & 0x1Fu) << 4;
-        // instruction descriptor fields the kernels are meant to set: D = F32 (bits 4-5 = 1), A = B = BF16 (bits 7-9, 10-12 = 1),
-        // no negate / transpose (K-major both), dense
-        if (((idesc >> 4) & 3u) != 1u || ((idesc >> 7) & 7u) != 1u || ((idesc >> 10) & 7u) != 1u) fail("tcgen05.mma: unexpected operand formats in the instruction descriptor");
-        if ((idesc >> 13) & 0xFu) fail("tcgen05.mma: negate / transpose bits set (the kernels use K-major operands)");
-        if (M != 128 || N < 16 || N > 256 || (N % 16)) fail("tcgen05.mma: M must be 128 and N a multiple of 16 up to 256");
-        const int lane0 = (int)(tm >> 16), col0 = (int)(tm & 0xFFFFu);
-        if (lane0 != 0 || col0 + N > g_tmem_cols) fail("tcgen05.mma: accumulator outside the allocated TMEM columns");
-        auto dec = [&](uint64_t d, uint64_t& start, uint64_t& sbo) {
+    if (has("wgmma.mma_async")) {
+        if (!has(".f32.bf16.bf16") || !has("m64n") || !has("p, 1, 1, 0, 0")) fail("wgmma: only m64nNk16.f32.bf16.bf16, unscaled, K-major operands are modelled");
+        const int N = atoi(strstr(text, "m64n") + 4);
+        if (N < 8 || N > 256 || (N % 8)) fail("wgmma: N must be a multiple of 8 up to 256");
+        if (n_out != N / 2 || n_in != 3) fail("wgmma: an m64nNk16 fp32 accumulator fragment is N / 2 registers per thread");
+        const uint64_t da = in[0], db = in[1];
+        const bool acc = in[2] != 0;
+        auto dec = [&](uint64_t d, uint64_t& start) {
             start = (d & 0x3FFFu) << 4;
-            sbo = ((d >> 32) & 0x3FFFu) << 4;
-            if ((d >> 61) != 2u) fail("tcgen05.mma: shared-memory descriptor is not SWIZZLE_128B");
-            if (((d >> 46) & 3u) != 1u) fail("tcgen05.mma: shared-memory descriptor version field is not 1 (sm_100)");
-            if (sbo != 1024) fail("tcgen05.mma: stride-byte-offset of a K-major SWIZZLE_128B tile must be 1024 (8 rows x 128 B)");
-            if ((start & ~(uint64_t)127) % 1024) fail("tcgen05.mma: swizzled operand tile is not 1024-byte aligned");
+            const uint64_t sbo = ((d >> 32) & 0x3FFFu) << 4;
+            if ((d >> 62) != 1u) fail("wgmma: shared-memory descriptor is not SWIZZLE_128B (layout type 1)");
+            if ((d >> 49) & 7u) fail("wgmma: base offset set (the kernels use 1024-byte aligned tiles)");
+            if (sbo != 1024) fail("wgmma: stride-byte-offset of a K-major SWIZZLE_128B tile must be 1024 (8 rows x 128 B)");
+            if ((start & ~(uint64_t)127) % 1024) fail("wgmma: swizzled operand tile is not 1024-byte aligned");
         };
-        uint64_t sa, sboa, sb, sbob;
-        dec(da, sa, sboa);
-        dec(db, sb, sbob);
-        auto elem = [&](uint64_t start, uint64_t sbo, int row, int k) {
-            const uint64_t a = swz128(start + (uint64_t)(row / 8) * sbo + (uint64_t)(row % 8) * 128 + (uint64_t)k * 2);
+        uint64_t sa, sb;
+        dec(da, sa);
+        dec(db, sb);
+        auto elem = [&](uint64_t start, int row, int k) {
+            const uint64_t a = swz128(start + (uint64_t)(row / 8) * 1024 + (uint64_t)(row % 8) * 128 + (uint64_t)k * 2);
             uint16_t v;
             memcpy(&v, smem_at(a, 2), 2);
             return bf16(v);
         };
-        float av[128][16];
-        for (int i = 0; i < M; ++i)
-            for (int k = 0; k < 16; ++k) av[i][k] = elem(sa, sboa, i, k);
-        for (int j = 0; j < N; ++j) {
-            float bv[16];
-            for (int k = 0; k < 16; ++k) bv[k] = elem(sb, sbob, j, k);
-            for (int i = 0; i < M; ++i) {
-                uint32_t& cell = g_tmem[(size_t)i * 512 + col0 + j];
-                float d;
-                memcpy(&d, &cell, 4);
-                if (!acc) d = 0.f;
-                for (int k = 0; k < 16; ++k) d += av[i][k] * bv[k];
-                memcpy(&cell, &d, 4);
-            }
+        const int w = cur->warp % 4, l = cur->lane;
+        for (int j = 0; j < N / 2; ++j) {          // the thread's fragment (tc_common.cuh: frag_row / frag_col)
+            const int row = 16 * w + l / 4 + 8 * ((j / 2) % 2), col = 8 * (j / 4) + 2 * (l % 4) + j % 2;
+            if (out_sizes[j] != 4) fail("wgmma: accumulator registers are 32-bit");
+            float d;
+            memcpy(&d, outs[j], 4);
+            if (!acc) d = 0.f;
+            for (int k = 0; k < 16; ++k) d += elem(sa, row, k) * elem(sb, col, k);
+            memcpy(outs[j], &d, 4);
         }
         note_progress();
-        return;
-    }
-    if (has("tcgen05.commit")) {
-        bar_arrive(bar_at(in[0]));               // every MMA issued so far has already executed in this model
-        return;
-    }
-    if (has("tcgen05.ld") && has("32x32b.x32")) {
-        if (n_out != 32) fail("tcgen05.ld.32x32b.x32 needs 32 destination registers");
-        const uint32_t ta = (uint32_t)in[0];
-        const int lane_base = (int)(ta >> 16), col0 = (int)(ta & 0xFFFFu);
-        if (lane_base != (cur->warp % 4) * 32) fail("tcgen05.ld: a warp may only access the TMEM lane quarter 32 * (warp % 4)");
-        if (col0 + 32 > g_tmem_cols) fail("tcgen05.ld beyond the allocated TMEM columns");
-        for (int j = 0; j < 32; ++j) out32(outs, out_sizes, j, g_tmem[(size_t)(lane_base + cur->lane) * 512 + col0 + j]);
         return;
     }
     if (has("multimem.ld_reduce") && has("add.v4.f32")) {

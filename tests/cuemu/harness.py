@@ -31,7 +31,7 @@ def emu_lib():
             try:
                 fn = getattr(lib, name)
             except AttributeError:
-                continue                      # entry points of files the emulator cannot compile (CUB, TMA, tcgen05)
+                continue                      # entry points of files the emulator cannot compile (CUB, TMA, wgmma)
             fn.restype, fn.argtypes = res, args
             have.append(name)
         lib._emulated = tuple(have)

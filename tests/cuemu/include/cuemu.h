@@ -15,8 +15,7 @@
 //   * a block in which every live fiber waits at a barrier that cannot complete is reported as a deadlock
 //     (divergent __syncthreads, a shuffle mask naming a lane that went elsewhere).
 //   * inline PTX is routed to cuemu_ptx.cpp: a functional model of the subset the tensor-core kernels use (mbarrier, 2-D
-//     TMA tensor copies with the 128-byte swizzle, tcgen05 alloc / mma / commit / ld, TMEM), calibrated on the kernel
-//     that is parity-green on real B200s; anything else (multimem, 1-D bulk copies) fails the launch;
+//     TMA tensor copies with the 128-byte swizzle, wgmma with register accumulators); anything else fails the launch;
 //   * CUB's two device primitives are host shims.
 // It proves indexing, reduction order, barrier / pipeline protocol and the host-side argument marshalling; it says nothing
 // about performance, memory coalescing, true asynchrony or device math rounding.  Nothing under mmssl_b200/ includes this.
@@ -103,8 +102,8 @@ void exchange_begin(unsigned mask, uint64_t bits);   // deposit + barrier
 uint64_t exchange_peek(int lane, bool* valid);
 void exchange_end(unsigned mask);
 // Inline PTX, as rewritten by build.py: template text, pointers to / sizes of the outputs, the inputs as 64-bit values.
-// cuemu_ptx.cpp models the subset the library uses (mbarrier, 2-D TMA tensor copies with the 128-byte swizzle, tcgen05
-// alloc / mma kind::f16 / commit / ld 32x32b, griddepcontrol) and fails the launch on anything else (multimem, ...).
+// cuemu_ptx.cpp models the subset the library uses (mbarrier, TMA copies with the 128-byte swizzle, wgmma m64nNk16 bf16,
+// multimem over registered replica groups, griddepcontrol) and fails the launch on anything else.
 void ptx_op(const char* text, void** outs, const int* out_sizes, int n_out, const uint64_t* ins, int n_in);
 void ptx_block_reset();
 void yield_blocked();                                 // give the CPU to the other fibers of the block (a failed try_wait)
@@ -161,7 +160,7 @@ static inline cudaError_t cudaMemset(void* p, int v, size_t n) { memset(p, v, n)
 static inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t = nullptr) { memmove(d, s, n); return cudaSuccess; }
 static inline cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { memmove(d, s, n); return cudaSuccess; }
 static inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
-static inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr a, int) { *v = a == cudaDevAttrMultiProcessorCount ? 148 : 10; return cudaSuccess; }
+static inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr a, int) { *v = a == cudaDevAttrMultiProcessorCount ? 132 : 9; return cudaSuccess; }
 template <typename F> static inline cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int* n, F, int, size_t) { *n = 8; return cudaSuccess; }
 static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
 static inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }

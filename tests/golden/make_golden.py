@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Mint golden vectors from the UNMODIFIED reference (/root/reference/MMSSL), run on CPU.
+"""Mint golden vectors from the UNMODIFIED reference (a checkout of HKUDS/MMSSL named by $MMSSL_REFERENCE), run on CPU.
 
-Runs only in the build container (the GPU box has no /root/reference).  One sub-process per case
+Runs only where that checkout exists; the tests read the stored vectors.  One sub-process per case
 because the reference parses its CLI flags at import time in four modules.
 
     python tests/golden/make_golden.py            # writes tests/golden/case_*.npz
@@ -23,7 +23,7 @@ import numpy as np
 import scipy.sparse as sp
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference/MMSSL"
+REF = os.environ.get("MMSSL_REFERENCE", "MMSSL")      # the directory holding the reference's main.py
 
 CASES = {
     # name: (n_users, n_items, dv, dt, batch, weight_size, graph mode, train mode, seed)

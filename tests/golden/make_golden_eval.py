@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Mint golden vectors for the evaluation path (SURVEY section 8f row 3) from the UNMODIFIED reference
-(/root/reference/MMSSL/utility/batch_test.py + metrics.py), run on CPU in the build container.
+(utility/batch_test.py + metrics.py of the checkout named by $MMSSL_REFERENCE), run on CPU.
 
     python tests/golden/make_golden_eval.py        # writes tests/golden/eval_*.npz
 
@@ -22,7 +22,7 @@ import numpy as np
 import scipy.sparse as sp
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference/MMSSL"
+REF = os.environ.get("MMSSL_REFERENCE", "MMSSL")      # the directory holding the reference's main.py
 
 CASES = {
     # random fp32 embeddings: almost no exact ties

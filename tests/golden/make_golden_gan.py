@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Mint a golden TRACE of the reference's full training step (GAN side included, SURVEY section 8f row 2) by running
-the UNMODIFIED `Trainer.train()` of /root/reference/MMSSL/main.py for three steps on CPU and recording what flows
-through it.  Build-container only (the GPU box has no /root/reference).
+the UNMODIFIED `Trainer.train()` of the reference's main.py ($MMSSL_REFERENCE) for three steps on CPU and recording what flows
+through it.  Runs only where that checkout exists.
 
     python tests/golden/make_golden_gan.py        # writes tests/golden/gan_trace.npz
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Records what the UNMODIFIED reference sampler (utility/load_data.py:Data.sample, :153-191) draws on
 tests/golden/dataset_small for fixed seeds of `random` and `numpy.random` -> tests/golden/sampler_small.json.
-Build-container only (imports /root/reference)."""
+Runs only where the reference checkout ($MMSSL_REFERENCE) exists."""
 import json
 import os
 import random

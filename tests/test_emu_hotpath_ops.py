@@ -1,4 +1,4 @@
-"""Kernels of the hot path that are already parity-green on a real B200 (tests/test_gpu_ops.py), executed on the CPU by
+"""Kernels of the hot path that are parity-green on a real H100 (tests/test_gpu_ops.py), executed on the CPU by
 the cuemu fiber emulator through the same bodies.  Two purposes: (1) cross-check the emulator itself against kernels
 whose GPU behaviour is known -- warp-group shuffles, block reductions, 128-bit vector atomics, last-arriver counters;
 (2) keep these kernels under test in the `-m "not gpu"` suite, which runs where there is no GPU."""

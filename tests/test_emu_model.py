@@ -1,6 +1,6 @@
 """The whole hot path on the CPU: drop-in ``Models.MMSSL`` (autograd wrappers), the fused ``HotStep`` and three AdamW steps,
 executed by the cuemu fiber emulator (tests/cuemu) against the golden vectors minted from the unmodified reference -- the
-bodies of tests/test_gpu_model.py.  The tcgen05 GEMM is replaced by a host statement of its contract
+bodies of tests/test_gpu_model.py.  The wgmma GEMM is replaced by a host statement of its contract
 (tests/cuemu/gemm_bf16x3_host.cpp: bf16 hi/lo operands, split-K partials), every other kernel is the real source."""
 import pytest
 

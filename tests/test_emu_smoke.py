@@ -1,4 +1,4 @@
-"""__graft_entry__.smoke() (the driver's one-call check on a B200) executed on the CPU emulator: the same function, the same
+"""__graft_entry__.smoke() (the one-call end-to-end check on an H100) executed on the CPU emulator: the same function, the same
 oracle comparison, the emulated library in place of the CUDA one."""
 from tests.cuemu import harness
 

@@ -1,8 +1,8 @@
-"""The tcgen05 / TMA kernels executed on the CPU through cuemu's functional model of the PTX they issue (tests/cuemu/cuemu_ptx.cpp:
+"""The wgmma / TMA kernels executed on the CPU through cuemu's functional model of the PTX they issue (tests/cuemu/cuemu_ptx.cpp:
 mbarrier phases and transaction counts, 2-D TMA box copies with out-of-bounds zero fill and the 128-byte swizzle, UMMA
-shared-memory / instruction descriptors, TMEM, tcgen05.mma / commit / ld).
+shared-memory descriptors, wgmma accumulator fragments).
 
-  * calibration: csrc/proj_tc.cu -- parity-green on real B200s -- computes the right products through the model, for its three
+  * calibration: csrc/proj_tc.cu -- parity-green on the H100 -- computes the right products through the model, for its three
     tile widths, with split-K, ragged M and K;
   * csrc/gemm_wide.cu -- written without GPU access, shares tc_common.cuh's descriptor / swizzle / pipeline helpers with the
     kernel above -- is then checked in what is its own: tiling over N, out-of-bounds rows and columns, the alpha / accumulate
@@ -34,7 +34,7 @@ def test_wide_gemm_kernel_through_the_ptx_model(emu, monkeypatch, m, n, k):
 @pytest.mark.parametrize("chunk", [1, 2, 3])
 @pytest.mark.parametrize("m,n,k", [(130, 257, 200), (64, 24, 330)])
 def test_wide_gemm_multi_pass_accumulation(emu, chunk, m, n, k):
-    """The K range cut into several TMEM passes (two accumulator buffers, epilogue folds each pass into C): same result."""
+    """The K range cut into several accumulation passes (the epilogue folds each pass into C): same result."""
     from mmssl_b200 import ops
     from tests import test_gpu_zzz_gemm_wide as W
     ops.gemm_wide_set_chunk(chunk)

@@ -1,5 +1,5 @@
 """2-GPU test of the row-sharded propagation with the all-gather fused into the SpMM epilogue
-(symmetric memory + multimem.st).  Skipped on single-GPU boxes; run with `gpurun --gpus 2`."""
+(symmetric memory + multimem.st).  Skipped on single-GPU machines."""
 import json
 import os
 import subprocess

@@ -80,7 +80,7 @@ def test_full_size_hot_step_vs_oracle(name, modal, batch):
     from mmssl_b200.engine import LIVE
     from mmssl_b200.hotstep import HotStep, HotStepConfig
     from mmssl_b200.synthetic import TripleSampler
-    torch.set_num_threads(8)         # torch's CPU sparse kernels collapse with more threads (profiles/r01_cpu_threads.txt)
+    torch.set_num_threads(8)         # torch's CPU sparse kernels collapse with more threads (tools/cpu_threads.py)
     dev = torch.device("cuda")
     ds, P, feats, graphs, feats_cpu = bench.build_problem(name, 2022, dev)
     ui, iu = O.to_torch_coo(ds.ui_norm), O.to_torch_coo(ds.iu_norm)

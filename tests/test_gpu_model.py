@@ -150,7 +150,7 @@ def test_hot_step_graph_replay_and_adamw_vs_oracle():
 
 @pytest.mark.parametrize("d,modal", [(128, "random"), (256, "random"), (128, "alias"), (64, "random")])
 def test_hot_step_other_widths_vs_oracle(d, modal):
-    """d = 128 / 256 code paths (32-lane SpMM groups, N=128/256 tcgen05 tiles, GEMM-path id fusion at 256)
+    """d = 128 / 256 code paths (32-lane SpMM groups, N=128/256 wgmma tiles, GEMM-path id fusion at 256)
     against the oracle (itself pinned to the reference) on a fresh synthetic problem."""
     import scipy.sparse as sp
     from oracle import mmssl_oracle as O

@@ -1,5 +1,5 @@
 """Per-kernel parity of libmmssl_b200 against CPU restatements (scipy / torch-CPU fp64).  All tests
-call through the C ABI (ctypes) on a real B200."""
+call through the C ABI (ctypes) on a real H100."""
 import math
 
 import numpy as np
@@ -140,7 +140,7 @@ def test_spmm_tma_hot_rows(d, nrhs):
     b = ops.spmm(g.fwd, xs, cs=cs, alpha=0.5, epilogue=ops.EPI_SOFTMAX, impl=ops.SPMM_IMPL_TMA)
     for u, w in zip(a, b):
         # the three heavy rows (~6.7k non-zeros, |logit| ~ 80) are reduced with float atomics in arrival order: an fp32 sum of
-        # 6.7k terms moves by ~3e-4 between orders, and a softmax output by up to a quarter of that (measured on B200: 1.1e-5 in
+        # 6.7k terms moves by ~3e-4 between orders, and a softmax output by up to a quarter of that (measured on the earlier hardware: 1.1e-5 in
         # the suite, 7e-5 under compute-sanitizer's timing).  The plain products above are held to 1e-5.
         assert rel_err(w, u) < 2e-4
     yt = ops.spmm(g.bwd, [torch.randn(n_rows, d, device="cuda")], impl=ops.SPMM_IMPL_TMA)[0]   # A^T: hot set = heavy rows of A
@@ -224,7 +224,7 @@ def test_sgemm(ta, tb):
 
 @pytest.mark.parametrize("m,n,k", [(300, 64, 96), (7050, 64, 1024), (1000, 128, 520), (515, 256, 200), (4096, 64, 7050)])
 def test_gemm_bf16x3_tensor_core(m, n, k):
-    """tcgen05 projection GEMM vs fp64: the bf16 hi/lo split must deliver fp32-level accuracy."""
+    """wgmma projection GEMM vs fp64: the bf16 hi/lo split must deliver fp32-level accuracy."""
     from mmssl_b200 import ops
     torch.manual_seed(3)
     a = torch.randn(m, k, device="cuda")

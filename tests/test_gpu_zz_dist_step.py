@@ -1,4 +1,4 @@
-"""2-GPU test of the row-sharded WHOLE hot step (sorts last; skipped on single-GPU boxes; run with `gpurun --gpus 2`)."""
+"""2-GPU test of the row-sharded WHOLE hot step (sorts last; skipped on single-GPU machines)."""
 import json
 import os
 import subprocess

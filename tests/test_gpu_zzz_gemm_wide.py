@@ -1,11 +1,11 @@
-"""General-width tcgen05 GEMM (csrc/gemm_wide.cu) against fp64, the GAN side running on it, and the CUDA-graph capture of the
-whole training iteration.  All of it has run green on a B200 (round 2); nothing here is gated any more.
+"""General-width wgmma GEMM (csrc/gemm_wide.cu) against fp64, the GAN side running on it, and the CUDA-graph capture of the
+whole training iteration.
 
 Tolerance of the GEMM: 2e-5 max-norm.  Error model: a bf16 hi+lo pair carries 2^-17 per operand (~4.6e-6 on these shapes, the
 floor the short accumulation passes reach), plus the tensor core's fp32 accumulate, which is not round-to-nearest and grows
-linearly with the number of MMAs chained into one TMEM accumulator (measured: 2.8e-5 at 1323 chained MMAs, 9e-6 at 384): the
-kernel bounds a pass to 192 and folds passes into C with fp32 adds -> 6.6e-6 at K = 7050; fp32 cuBLAS gives 3.9e-6 on the same
-inputs (tools/gemm_wide_sweep.py, profiles/r02_gemm_wide_sweep.txt)."""
+with the number of MMAs chained into one accumulator (H100 80GB HBM3: 2.8e-5 at 1323 chained MMAs, 8.9e-6 at 384): the
+kernel bounds a pass to 192 and folds passes into C with fp32 adds -> 6.6e-6 at K = 7050; fp32 cuBLAS gives 8.3e-7 on the same
+inputs (tools/gemm_wide_sweep.py, DESIGN section 6)."""
 import pytest
 import torch
 

@@ -1,5 +1,5 @@
 """Thread-count sweep of the CPU baseline (bench.py's cpu_baseline leg): torch's sparse kernels get slower with more threads on
-the GPU boxes' hosts, so the baseline is reported at its best setting (profiles/r01_cpu_threads.txt)."""
+the GPU hosts, so the baseline is reported at its best setting."""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
 import bench

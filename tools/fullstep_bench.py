@@ -4,8 +4,7 @@ SURVEY 8d: "also report full step for C1-C3".  Prints one JSON line.
 
     python tools/fullstep_bench.py [config=baby] [--steps K] [--warmup W] [--gemm tc|simt|cublas] [--cpu-steps N]
 
-Not part of bench.py's contract (the headline metric is the hot step); written when round 1 had no GPU time left -- first run
-is a round-2 task (DESIGN section 9)."""
+Not part of bench.py's contract (the headline metric is the hot step); H100 numbers in DESIGN section 6."""
 import argparse
 import json
 import os

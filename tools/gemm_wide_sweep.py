@@ -1,5 +1,5 @@
-"""Error and time of the wide tcgen05 GEMM (csrc/gemm_wide.cu) against the accumulation-pass length, next to fp32 cuBLAS.
-    python tools/gemm_wide_sweep.py          (under gpurun; prints one JSON line per shape)"""
+"""Error and time of the wide wgmma GEMM (csrc/gemm_wide.cu) against the accumulation-pass length, next to fp32 cuBLAS.
+    python tools/gemm_wide_sweep.py          (on the GPU; prints one JSON line per shape)"""
 import json
 import os
 import sys

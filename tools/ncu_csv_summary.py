@@ -1,6 +1,6 @@
 """Summarise an `ncu --page raw --csv` export: one block of headline metrics per captured kernel.
 
-    python tools/ncu_csv_summary.py gpurun_out/p2_step_baby_raw.csv [kernel-name-substring]"""
+    python tools/ncu_csv_summary.py <ncu --csv export> [kernel-name-substring]"""
 import csv
 import sys
 

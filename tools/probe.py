@@ -1,5 +1,5 @@
 """GPU probe: in-graph (warm) latency of kernel chains at small scale, SpMM throughput at large scale.
-Usage (under gpurun): python tools/probe.py [small] [large]"""
+Usage (on the GPU): python tools/probe.py [small] [large]"""
 import json
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -10,7 +10,7 @@ from mmssl_b200.graph import BipartiteGraph
 from mmssl_b200.synthetic import make_dataset, make_bipartite, csr_norm
 
 dev = torch.device("cuda")
-PEAK = 6489.3
+PEAK = 3350.0      # GB/s: H100 SXM data-sheet HBM3 bandwidth (the fraction below is of the data sheet, not of a measured peak)
 
 
 def graph_time(fn, reps=20, inner=1):
@@ -209,7 +209,7 @@ def pipe(name="baby"):
     for impl in (4, 6, 2):
         out[f"impl{impl}"] = forms(impl)
     for per_sm in (0, 2, 3, 4, 6, 8):
-        ops.spmm_pipe_set_blocks(per_sm * 148)
+        ops.spmm_pipe_set_blocks(per_sm * torch.cuda.get_device_properties(0).multi_processor_count)
         for pre in (0, 64):
             out[f"pipe_b{per_sm}_pre{pre}"] = forms(ops.SPMM_IMPL_PIPE | pre)
     ops.spmm_pipe_set_blocks(0)

@@ -1,6 +1,6 @@
 """One problem, the row-sharded whole hot step with ONE and with TWO streams (the modality branch beside the id / GCN branch,
 each with its own exchange barriers), same process, CUDA graph, CUDA-event timing, max over ranks.  One JSON line per variant
-(rank 0), also appended to gpurun_out/<tag>.jsonl as soon as it exists.
+(rank 0), also appended to out/<tag>.jsonl as soon as it exists.
 
     python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tools/rowshard_ab.py syn1m [sports] [--steps K] [--tag T]"""
 import json
@@ -57,8 +57,8 @@ for name in names:
             line = json.dumps({"config": name, "n_gpus": world, "streams": 2 if streams == "1" else 1, "ms_per_step": round(float(ms), 4),
                                "schedule": sh.schedule, "steps": steps})
             print(line, flush=True)
-            os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-            with open(os.path.join(ROOT, "gpurun_out", tag + ".jsonl"), "a") as f:
+            os.makedirs(os.path.join(ROOT, "out"), exist_ok=True)
+            with open(os.path.join(ROOT, "out", tag + ".jsonl"), "a") as f:
                 f.write(line + "\n")
         del sh, P
         torch.cuda.empty_cache()

@@ -45,8 +45,8 @@ res = {"config": name, "n_gpus": world, "scheme": "row-sharded whole hot step", 
 if check:
     # Parity of ONE step without the optimiser: the five loss terms and every live gradient (table gradients: the rank's rows).
     # Parameters after AdamW are NOT the yardstick: m / (sqrt(v) + eps) turns a 1e-9 difference in a gradient entry of size 1e-8
-    # into a full-size (lr) difference of the parameter -- measured round 2: gradients agree to 5e-6 where the parameters after two
-    # AdamW steps differ by 1e-2 (summation orders differ between the two schemes).  A loose bound on the parameters is kept.
+    # into a full-size (lr) difference of the parameter -- on the earlier hardware gradients agreed to 5e-6 where the parameters
+    # after two AdamW steps differed by 1e-2 (summation orders differ between the two schemes).  A loose bound on the parameters is kept.
     _, Pd, feats, graphs, _ = bench.build_problem(name, 2022, dev)
     hs = HotStep(Pd, feats, graphs, cfg, batch=B, optimizer_step=False)
     hs.masks = tuple(m.to(dev) for m in full_masks)

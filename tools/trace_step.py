@@ -1,5 +1,5 @@
 """Kernel timeline of the CUDA-graph-replayed hot step (CUPTI via torch.profiler): true in-graph
-durations, stream overlap and gaps.  Usage (gpurun): python tools/trace_step.py [config]"""
+durations, stream overlap and gaps.  Usage (on the GPU): python tools/trace_step.py [config]"""
 import collections, json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
