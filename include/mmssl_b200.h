@@ -296,6 +296,19 @@ int mmssl_eval_rank(const float* user_emb, int64_t ldu, const float* item_emb, i
                     const int64_t* held_indptr, const int64_t* held_indices, const int32_t* ks_host, int n_ks,
                     int32_t* ranked, float* ranked_scores, int32_t* hits, double* per_user, float* scores_out,
                     void* stream);
+/* Full mode (--test_flag full, batch_test.py:38-68, metrics.py:95-100): the same ranking outputs as mmssl_eval_rank,
+ * plus auc_per_user[n_eval] fp64 = roc_auc_score over the user's non-training items in [0, n_items), positives =
+ * distinct held-out ids among them, ties counted 1/2.  Reference quirks kept: NaN when there is one class only, 0 when
+ * the user has no candidate item or a candidate's score is NaN / inf.  Exact from integer pair counts.
+ * Workspace: users whose held-out row is longer than mmssl_eval_full_stage() keep their positives' keys in
+ * pos_ws[pos_ws_off[g] ...], a slot of next_pow2(row length) uint32; pos_ws_off[n_eval] is read only for those users
+ * (pos_ws may be NULL when there is none). */
+int mmssl_eval_full_stage(void);
+int mmssl_eval_rank_full(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
+                         const int64_t* users, int64_t n_eval, const int64_t* train_indptr, const int64_t* train_indices,
+                         const int64_t* held_indptr, const int64_t* held_indices, const int32_t* ks_host, int n_ks,
+                         int32_t* ranked, float* ranked_scores, int32_t* hits, double* per_user, float* scores_out,
+                         double* auc_per_user, uint32_t* pos_ws, const int64_t* pos_ws_off, void* stream);
 int mmssl_eval_reduce(const double* per_user, int64_t n_eval, int n_metrics, double* result, void* stream);
 
 /* ------------------------------------------------------------------ GAN side (SURVEY 8f "next" #2), see csrc/gan.cu

@@ -70,6 +70,7 @@ class TrainerArgs:
     early_stopping_patience: int = 7    # :11
     feat_reg_decay: float = 1e-5        # :29
     mess_dropout: str = "[0.1, 0.1]"    # :13
+    test_flag: str = "part"             # :16
 
 
 def set_seed(seed: int) -> None:
@@ -145,7 +146,8 @@ class Trainer:
         cfg = FullStepConfig(hot=hot, gan=hp, m_topk_rate=args.m_topk_rate, T=args.T, G_drop1=args.G_drop1, G_drop2=args.G_drop2)
         self.step = FullStep(self.P, self.d_state, self.model._feature_stores(), t64(R.indptr), t64(R.indices), self.ui_graph,
                              self.iu_graph, cfg, batch=args.batch_size)
-        self.evaluator = Evaluator(data.train_items, data.test_set, data.val_set, self.n_users, self.n_items, self.Ks, device=dev)
+        self.evaluator = Evaluator(data.train_items, data.test_set, data.val_set, self.n_users, self.n_items, self.Ks, device=dev,
+                                   test_flag=args.test_flag)
         if sampler == "device":
             from .sampler import DeviceTripleSampler
             self._dev_sampler = DeviceTripleSampler(R, device=dev, seed=args.seed)
