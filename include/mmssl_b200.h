@@ -289,8 +289,10 @@ int mmssl_sample_triples(const int64_t* indptr, const int64_t* indices, const in
  *   hits[n_eval, kmax] 1/0 membership in the held-out row (CSR, SORTED), -1 past the end (may be NULL);
  *   per_user[n_eval, 4, n_ks] fp64 = precision, recall, ndcg, hit_ratio at every K (reference quirks kept:
  *   ideal DCG from the retrieved hit list, precision divisor shrinks with short lists, recall / len(held-out));
- *   scores_out[n_eval, n_items] (may be NULL; debugging / tests).  ks_host is a HOST array of n_ks <= 8 cut-offs <= 64.
- * mmssl_eval_reduce: result[m] = mean over users of per_user[:, m] (batch_test.py:159-163), fixed order. */
+ *   scores_out[n_eval, n_items] (may be NULL; debugging / tests).  ks_host is a HOST array of n_ks cut-offs;
+ *   mmssl_eval_rank / _full take 1..8 cut-offs in 1..64, mmssl_eval_rank_wide any number of cut-offs in 1..2^26.
+ *   kmax = max(Ks); the hit list has min(kmax, #non-training items) entries.
+ * mmssl_eval_reduce: result[m] = mean over users of per_user[:, m] (batch_test.py:159-163), fixed order, any n_metrics. */
 int mmssl_eval_rank(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
                     const int64_t* users, int64_t n_eval, const int64_t* train_indptr, const int64_t* train_indices,
                     const int64_t* held_indptr, const int64_t* held_indices, const int32_t* ks_host, int n_ks,
@@ -309,6 +311,18 @@ int mmssl_eval_rank_full(const float* user_emb, int64_t ldu, const float* item_e
                          const int64_t* held_indptr, const int64_t* held_indices, const int32_t* ks_host, int n_ks,
                          int32_t* ranked, float* ranked_scores, int32_t* hits, double* per_user, float* scores_out,
                          double* auc_per_user, uint32_t* pos_ws, const int64_t* pos_ws_off, void* stream);
+/* Wide path: the same outputs for any Ks (more than 8 cut-offs, K > 64, K > n_items).  ks_host (validation, sizing) and
+ * ks_dev (read by the kernel) hold the same n_ks cut-offs.  auc_per_user == NULL: part mode; else full mode with
+ * pos_ws / pos_ws_off as in mmssl_eval_rank_full.  Per-user candidate buffers hold cap = 2 ksel + 256 (rounded up to 128)
+ * keys, ksel = min(kmax, n_items): in shared memory while a CTA's 8 buffers and user vectors fit in 112 KiB, else in
+ * key_ws, which must hold mmssl_eval_wide_workspace_bytes(n_eval, kmax, n_items, d) bytes (0 in the shared-memory case):
+ * one slot of 8 cap keys per CTA, at most 528 slots and at most 512 MiB (at least one slot). */
+int64_t mmssl_eval_wide_workspace_bytes(int64_t n_eval, int kmax, int64_t n_items, int d);
+int mmssl_eval_rank_wide(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
+                         const int64_t* users, int64_t n_eval, const int64_t* train_indptr, const int64_t* train_indices,
+                         const int64_t* held_indptr, const int64_t* held_indices, const int32_t* ks_host, const int32_t* ks_dev,
+                         int n_ks, int32_t* ranked, float* ranked_scores, int32_t* hits, double* per_user, float* scores_out,
+                         double* auc_per_user, uint32_t* pos_ws, const int64_t* pos_ws_off, uint64_t* key_ws, void* stream);
 int mmssl_eval_reduce(const double* per_user, int64_t n_eval, int n_metrics, double* result, void* stream);
 
 /* ------------------------------------------------------------------ GAN side (SURVEY 8f "next" #2), see csrc/gan.cu

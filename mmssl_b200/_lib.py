@@ -105,6 +105,9 @@ _SIGS = {
     "mmssl_eval_full_stage": (C.c_int, []),
     "mmssl_eval_rank_full": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, C.POINTER(c_i32),
                                        c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "mmssl_eval_wide_workspace_bytes": (c_i64, [c_i64, c_i32, c_i64, c_i32]),
+    "mmssl_eval_rank_wide": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, C.POINTER(c_i32),
+                                       c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "mmssl_eval_reduce": (C.c_int, [c_vp, c_i64, c_i32, c_vp, c_vp]),
     "mmssl_gan_bn_fwd": (C.c_int, [c_vp] * 7 + [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp]),
     "mmssl_gan_bn_bwd": (C.c_int, [c_vp] * 5 + [c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp]),
@@ -154,7 +157,7 @@ KERNELS_PER_CALL = {
     "mmssl_infonce_stats": 2, "mmssl_infonce_grad": 1, "mmssl_infonce_scatter": 1, "mmssl_infonce_stats_tc": 4, "mmssl_infonce_forward_tc": 3, "mmssl_infonce_grad_tc": 1, "mmssl_loss_assemble": 1,
     "mmssl_step_tick": 1, "mmssl_dp_fused_adamw": 1, "mmssl_dp_fused_adamw_dev": 1, "mmssl_sampler_init": 1, "mmssl_sample_triples": 1, "mmssl_adamw": 1, "mmssl_split_bf16": 1, "mmssl_split_bf16_t": 1, "mmssl_split_bf16_t_colsum": 1, "mmssl_gemm_bf16x3": 1, "mmssl_gemm_bf16x3_wide": 1,
     "mmssl_proj_epilogue": 1, "mmssl_wgrad_epilogue": 1, "mmssl_colsum": 1,
-    "mmssl_eval_rank": 1, "mmssl_eval_rank_full": 1, "mmssl_eval_reduce": 1,
+    "mmssl_eval_rank": 1, "mmssl_eval_rank_full": 1, "mmssl_eval_rank_wide": 1, "mmssl_eval_reduce": 1,
     "mmssl_gan_bn_fwd": 1, "mmssl_gan_bn_bwd": 1, "mmssl_gan_gp_rev_bn": 1, "mmssl_gan_bn_fwd_rev": 1, "mmssl_gan_colsum": 1,
     "mmssl_gan_head_fwd": 2, "mmssl_gan_head_bwd": 1, "mmssl_gan_gp_rows": 2, "mmssl_gan_gp_head_rev": 2, "mmssl_gan_usim_finish": 1,
     "mmssl_gan_usim_bwd_pre": 1, "mmssl_gan_real_rows": 1, "mmssl_gan_interpolate": 1, "mmssl_gan_add_scaled": 1,

@@ -4,7 +4,8 @@
 ranks them in a ``multiprocessing.Pool`` with ``heapq`` (batch_test.py:112-169); here ranking, masking of the
 training items, hit marking and the metrics are one kernel and only the [4, len(Ks)] result leaves the GPU.
 ``test_flag='full'`` (batch_test.py:38-68, 104-107) adds the per-user ROC-AUC over all non-training items
-(``mmssl_eval_rank_full``): the same sweep, no host sort."""
+(``mmssl_eval_rank_full``): the same sweep, no host sort.  Ks is any list of cut-offs >= 1 (parser.py:63), unsorted or with
+duplicates: up to 8 cut-offs of at most 64 go to the shared-memory kernel, any other list to ``mmssl_eval_rank_wide``."""
 from __future__ import annotations
 
 import ctypes as C
@@ -44,13 +45,16 @@ class Evaluator:
         _lib.load(require_device=True)
         self.n_users, self.n_items = int(n_users), int(n_items)
         self.Ks = [int(k) for k in Ks]
-        if not (1 <= len(self.Ks) <= 8 and all(1 <= k <= 64 for k in self.Ks)):
-            raise ValueError("Ks: 1..8 cut-offs, each in 1..64")
+        if not self.Ks or min(self.Ks) < 1:
+            raise ValueError("Ks: at least one cut-off, each >= 1")
+        # the kernel with 512-key shared buffers and a 64-bit hit mask takes up to 8 cut-offs of at most 64
+        self.wide = len(self.Ks) > 8 or max(self.Ks) > 64
         self.device = torch.device(device)
         self.train = _rows_to_csr(train_items, n_users, self.device)
         self.held = {False: _rows_to_csr(test_set, n_users, self.device), True: _rows_to_csr(val_set, n_users, self.device)}
         self._held_len = {k: np.diff(v[0].cpu().numpy()) for k, v in self.held.items()}
         self._ks = (C.c_int32 * len(self.Ks))(*self.Ks)
+        self._ks_dev = torch.tensor(self.Ks, dtype=torch.int32).to(self.device) if self.wide else None
 
     def rank(self, ua_embeddings: torch.Tensor, ia_embeddings: torch.Tensor, users_to_test, is_val: bool,
              want_scores: bool = False) -> Dict[str, torch.Tensor]:
@@ -81,9 +85,12 @@ class Evaluator:
         result = torch.zeros(4, nk, dtype=torch.float64, device=dev)
         scores = torch.empty(n, self.n_items, dtype=torch.float32, device=dev) if want_scores else None
         held = self.held[bool(is_val)]
-        args = (ptr(ua), ua.stride(0), ptr(ia), ia.stride(0), self.n_items, d, ptr(users), n, ptr(self.train[0]), ptr(self.train[1]),
-                ptr(held[0]), ptr(held[1]), self._ks, nk, ptr(ranked), ptr(rscore), ptr(hits), ptr(per_user), ptr(scores))
+        head = (ptr(ua), ua.stride(0), ptr(ia), ia.stride(0), self.n_items, d, ptr(users), n, ptr(self.train[0]), ptr(self.train[1]),
+                ptr(held[0]), ptr(held[1]), self._ks)
+        ks = (ptr(self._ks_dev), nk) if self.wide else (nk,)
+        args = head + ks + (ptr(ranked), ptr(rscore), ptr(hits), ptr(per_user), ptr(scores))
         out = dict(ranked=ranked, ranked_scores=rscore, hits=hits, per_user=per_user, result=result)
+        auc = ws = off = None
         if self.test_flag == "full":
             # users whose held-out row does not fit the kernel's shared-memory stage sort their positives in a
             # workspace slot of next_pow2(row length) keys
@@ -94,8 +101,13 @@ class Evaluator:
             off = torch.from_numpy(np.cumsum(slot) - slot).to(dev)
             ws = torch.empty(int(slot.sum()), dtype=torch.int32, device=dev) if slot.sum() else None
             auc = torch.empty(n, dtype=torch.float64, device=dev)
-            _lib.check(lib.mmssl_eval_rank_full(*args, ptr(auc), ptr(ws), ptr(off), stream()))
             out["auc"] = auc
+        if self.wide:
+            nbytes = lib.mmssl_eval_wide_workspace_bytes(n, kmax, self.n_items, d)
+            key_ws = torch.empty(nbytes // 8, dtype=torch.int64, device=dev) if nbytes else None
+            _lib.check(lib.mmssl_eval_rank_wide(*args, ptr(auc), ptr(ws), ptr(off), ptr(key_ws), stream()))
+        elif self.test_flag == "full":
+            _lib.check(lib.mmssl_eval_rank_full(*args, ptr(auc), ptr(ws), ptr(off), stream()))
         else:
             _lib.check(lib.mmssl_eval_rank(*args, stream()))
         _lib.check(lib.mmssl_eval_reduce(ptr(per_user), n, 4 * nk, ptr(result), stream()))

@@ -3,7 +3,10 @@ drawn from a seed, random fp32 embeddings) in part mode (top-K ranking + metrics
 per-user ROC-AUC over all non-training items), timed with CUDA events after a warm-up.  Prints one JSON line with the
 card name and power limit read in the same run.
 
-    python tools/eval_bench.py [baby|sports|tiktok] [--iters N] [--warmup W]
+    python tools/eval_bench.py [baby|sports|tiktok] [--iters N] [--warmup W] [--ks "[10, 20, 50, 100]"]
+
+--ks takes the reference's --Ks syntax; up to 8 cut-offs of at most 64 use the shared-memory kernel, any other list the
+wide path (mmssl_eval_rank_wide).
 
 Not part of bench.py's contract; H100 numbers in DESIGN section 6."""
 import argparse
@@ -22,7 +25,9 @@ ap.add_argument("config", nargs="?", default="baby", choices=["tiktok", "baby", 
 ap.add_argument("--iters", type=int, default=20)
 ap.add_argument("--warmup", type=int, default=3)
 ap.add_argument("--seed", type=int, default=0)
+ap.add_argument("--ks", default="[10, 20, 50]")
 a = ap.parse_args()
+Ks = [int(k) for k in json.loads(a.ks)]
 
 from mmssl_b200.evaluate import Evaluator  # noqa: E402
 from mmssl_b200.synthetic import CONFIGS, make_bipartite  # noqa: E402
@@ -40,7 +45,7 @@ users = list(range(U))
 
 
 def time_mode(flag):
-    ev = Evaluator(train, held, {}, U, I, [10, 20, 50], test_flag=flag)
+    ev = Evaluator(train, held, {}, U, I, Ks, test_flag=flag)
     for _ in range(a.warmup):
         ev.rank(ua, ia, users, False)
     torch.cuda.synchronize()
@@ -57,7 +62,7 @@ part_ms, part = time_mode("part")
 full_ms, full = time_mode("full")
 same = all(torch.equal(part[k], full[k]) for k in ("ranked", "hits", "per_user"))
 q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-print(json.dumps(dict(config=a.config, users=U, items=I, d=d, iters=a.iters, part_ms=round(part_ms, 3), full_ms=round(full_ms, 3),
+print(json.dumps(dict(config=a.config, users=U, items=I, d=d, Ks=Ks, wide=bool(Evaluator(train, held, {}, U, I, Ks).wide), iters=a.iters, part_ms=round(part_ms, 3), full_ms=round(full_ms, 3),
                       full_over_part=round(full_ms / part_ms, 3), ranking_equal=same,
                       mean_auc=float(full["auc"].mean().item()), card=torch.cuda.get_device_name(),
                       nvidia_smi=q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else None)))
