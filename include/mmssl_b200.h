@@ -424,6 +424,27 @@ int64_t mmssl_gemm_bf16x3_workspace_floats(int64_t m, int64_t n, int64_t k, int*
 int mmssl_gemm_bf16x3(const uint16_t* a_hi, const uint16_t* a_lo, int64_t lda, const uint16_t* b_hi,
                       const uint16_t* b_lo, int64_t ldb, int64_t m, int64_t n, int64_t k, int split_k, float* partial,
                       void* stream);
+/* One problem of a grouped projection GEMM: the operands and result of mmssl_gemm_bf16x3. */
+typedef struct {
+    const uint16_t* a_hi;
+    const uint16_t* a_lo;
+    int64_t lda;
+    const uint16_t* b_hi;
+    const uint16_t* b_lo;
+    int64_t ldb;
+    int64_t m, n, k;
+    float* partial;   /* [split_k][m][n] */
+    int32_t split_k;
+    int32_t reserved;
+} mmssl_gemm_problem_t;
+/* Plan of a group of one or two problems (mnk = m0, n0, k0, m1, n1, k1; the same n): per problem the split count and the
+ * partial-buffer size in floats; optionally the units in the order the CTAs walk them, 4 int32 each
+ * (problem, m_tile, kb_begin, kb_end), at most units_cap of them.  max_ctas caps the grid (0 = one resident wave) and must
+ * be the value later passed to mmssl_gemm_bf16x3_group.  Returns the number of units, or -1 on bad arguments. */
+int64_t mmssl_gemm_bf16x3_group_plan(int n_problems, const int64_t* mnk, int max_ctas, int* split_out, int64_t* floats_out,
+                                     int32_t* units_out, int64_t units_cap);
+/* Every problem's partial[s][m][n] as mmssl_gemm_bf16x3 with the same split_k would write it, in ONE persistent launch. */
+int mmssl_gemm_bf16x3_group(int n_problems, const mmssl_gemm_problem_t* problems, int max_ctas, void* stream);
 /* General-width variant for the GAN side (gemm_wide.cu): c[m][ldc] = alpha * (Ahi+Alo)[m,k] * (Bhi+Blo)[n,k]^T (+ c when
  * accumulate != 0), any n >= 1, no split-K, alpha / accumulate applied in the epilogue; replaces the Discriminator's
  * nn.Linear products and their closed-form backward / gradient-penalty variants (Models.py:224-245, main.py:140-160). */

@@ -25,6 +25,12 @@ class CsrDesc(C.Structure):
                 ("segs_cap", c_i64)]
 
 
+class GemmProblem(C.Structure):
+    """mmssl_gemm_problem_t"""
+    _fields_ = [("a_hi", c_vp), ("a_lo", c_vp), ("lda", c_i64), ("b_hi", c_vp), ("b_lo", c_vp), ("ldb", c_i64),
+                ("m", c_i64), ("n", c_i64), ("k", c_i64), ("partial", c_vp), ("split_k", C.c_int32), ("reserved", C.c_int32)]
+
+
 class SpmmRhs(C.Structure):
     """mmssl_spmm_rhs_t"""
     _fields_ = [("x", c_vp), ("ldx", c_i64), ("y", c_vp), ("ldy", c_i64), ("c", c_vp), ("ldc", c_i64),
@@ -137,6 +143,8 @@ _SIGS = {
     "mmssl_split_bf16_t_colsum": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp]),
     "mmssl_gemm_bf16x3_workspace_floats": (c_i64, [c_i64, c_i64, c_i64, C.POINTER(c_i32)]),
     "mmssl_gemm_bf16x3": (C.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_i32, c_vp, c_vp]),
+    "mmssl_gemm_bf16x3_group_plan": (c_i64, [c_i32, C.POINTER(c_i64), c_i32, C.POINTER(c_i32), C.POINTER(c_i64), c_vp, c_i64]),
+    "mmssl_gemm_bf16x3_group": (C.c_int, [c_i32, C.POINTER(GemmProblem), c_i32, c_vp]),
     "mmssl_gemm_bf16x3_wide": (C.c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_f32, c_i32, c_vp, c_i64, c_vp]),
     "mmssl_gemm_wide_set_chunk": (C.c_int, [c_i32]),
     "mmssl_spmm_pipe_set_blocks": (C.c_int, [c_i32]),
@@ -155,7 +163,7 @@ KERNELS_PER_CALL = {
     "mmssl_dwcat_reduce": 1, "mmssl_combine_fwd": 1, "mmssl_combine_bwd": 1, "mmssl_softmax_bwd": 1,
     "mmssl_axpby": 1, "mmssl_mul_mask": 1, "mmssl_sumsq": 1, "mmssl_bpr": 1, "mmssl_infonce_prepare": 1,
     "mmssl_infonce_stats": 2, "mmssl_infonce_grad": 1, "mmssl_infonce_scatter": 1, "mmssl_infonce_stats_tc": 4, "mmssl_infonce_forward_tc": 3, "mmssl_infonce_grad_tc": 1, "mmssl_loss_assemble": 1,
-    "mmssl_step_tick": 1, "mmssl_dp_fused_adamw": 1, "mmssl_dp_fused_adamw_dev": 1, "mmssl_sampler_init": 1, "mmssl_sample_triples": 1, "mmssl_adamw": 1, "mmssl_split_bf16": 1, "mmssl_split_bf16_t": 1, "mmssl_split_bf16_t_colsum": 1, "mmssl_gemm_bf16x3": 1, "mmssl_gemm_bf16x3_wide": 1,
+    "mmssl_step_tick": 1, "mmssl_dp_fused_adamw": 1, "mmssl_dp_fused_adamw_dev": 1, "mmssl_sampler_init": 1, "mmssl_sample_triples": 1, "mmssl_adamw": 1, "mmssl_split_bf16": 1, "mmssl_split_bf16_t": 1, "mmssl_split_bf16_t_colsum": 1, "mmssl_gemm_bf16x3": 1, "mmssl_gemm_bf16x3_group": 1, "mmssl_gemm_bf16x3_wide": 1,
     "mmssl_proj_epilogue": 1, "mmssl_wgrad_epilogue": 1, "mmssl_colsum": 1,
     "mmssl_eval_rank": 1, "mmssl_eval_rank_full": 1, "mmssl_eval_rank_wide": 1, "mmssl_eval_reduce": 1,
     "mmssl_gan_bn_fwd": 1, "mmssl_gan_bn_bwd": 1, "mmssl_gan_gp_rev_bn": 1, "mmssl_gan_bn_fwd_rev": 1, "mmssl_gan_colsum": 1,

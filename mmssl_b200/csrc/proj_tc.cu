@@ -31,6 +31,8 @@ struct GemmCfg {
     static constexpr int kStages = (N == 64) ? 2 : (N == 128 ? 3 : 2);
     static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
+static constexpr int ctas_per_sm(int64_t n) { return n == 64 ? 2 : 1; }   // GemmCfg<n>::kCtasPerSm
+constexpr int kGroupMax = 2;                                                // problems of one grouped launch (image, text)
 
 template <int N>
 __global__ void __launch_bounds__(kThreads, GemmCfg<N>::kCtasPerSm)
@@ -126,6 +128,149 @@ static int launch_gemm(const CUtensorMap& ah, const CUtensorMap& al, const CUten
     return 0;
 }
 
+// ---- grouped, persistent variant: the image and text problems of one direction in one launch ----------------------------
+//
+// The work of a group is a list of units (problem, m_tile, K slice).  Each problem cuts its K into `split` slices of `per`
+// k-blocks (the last one may be shorter), exactly as the kernel above does for the same split, so a unit writes the same
+// partial[s][m][n] tile the single-problem kernel would.  One resident wave of CTAs walks the list: CTA b takes units
+// b, b + gridDim.x, ... (a static schedule: the same CTA computes the same tile on every launch).  The TMA producer runs
+// across unit boundaries: the stage ring and its mbarrier phases continue from one unit to the next, so the next unit's
+// stages land while the consumers store the previous unit's accumulators.
+//
+// The unit list is not stored: it is a few classes of equal-length units (per problem: its full slices, then its shorter
+// last slice), sorted longest first, and a unit's index decodes into (class, slice, m_tile) on the device and on the host.
+struct GroupClass {
+    float* partial;             // the problem's partial[split][m][n]
+    int prob, m, m_tiles, per;  // problem index, rows, 128-row tiles, k-blocks per full slice
+    int s0, u0, n_units, len;   // first slice of the class, first unit index, units (= slices * m_tiles), k-blocks per unit
+};
+struct GroupParams {
+    CUtensorMap maps[kGroupMax][4];   // a_hi, a_lo, b_hi, b_lo of each problem
+    GroupClass cls[2 * kGroupMax];
+    int n_classes, n_units, n_problems;
+};
+struct GroupUnit { int cls, slice, m_tile, kb0, kb1; };
+
+__host__ __device__ __forceinline__ GroupUnit group_unit(const GroupClass* cls, int n_classes, int u) {
+    int c = 0;
+    while (c + 1 < n_classes && u >= cls[c + 1].u0) ++c;
+    const GroupClass& k = cls[c];
+    const int j = u - k.u0;
+    GroupUnit w;
+    w.cls = c;
+    w.slice = k.s0 + j / k.m_tiles;
+    w.m_tile = j % k.m_tiles;
+    w.kb0 = w.slice * k.per;
+    w.kb1 = w.kb0 + k.len;
+    return w;
+}
+
+template <int N>
+__global__ void __launch_bounds__(kThreads, GemmCfg<N>::kCtasPerSm)
+gemm_bf16x3_group_kernel(const __grid_constant__ GroupParams P) {
+    using Cfg = GemmCfg<N>;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+    uint64_t* empty_bar = full_bar + Cfg::kStages;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp == kProducerWarp && lane == 0) {
+        for (int p = 0; p < P.n_problems; ++p)
+            for (int t = 0; t < 4; ++t) asm volatile("prefetch.tensormap [%0];" ::"l"(&P.maps[p][t]) : "memory");
+        for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerWarps); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp == kProducerWarp) {
+        if (lane == 0) {
+            int it = 0;   // k-blocks issued by this CTA so far: stage it % kStages, phase (it / kStages) & 1
+            for (int u = blockIdx.x; u < P.n_units; u += gridDim.x) {
+                const GroupUnit w = group_unit(P.cls, P.n_classes, u);
+                const CUtensorMap* tm = P.maps[P.cls[w.cls].prob];
+                const int y = w.m_tile * kBlockM;
+                for (int kb = w.kb0; kb < w.kb1; ++kb, ++it) {
+                    const int s = it % Cfg::kStages;
+                    mbar_wait(&empty_bar[s], ((uint32_t)(it / Cfg::kStages) & 1u) ^ 1u);
+                    uint8_t* st = smem + s * Cfg::kStageBytes;
+                    mbar_expect_tx(&full_bar[s], Cfg::kStageBytes);
+                    const int kx = kb * kBlockK;
+                    tma_load_2d(&tm[0], &full_bar[s], st, kx, y, kEvictFirst);
+                    tma_load_2d(&tm[1], &full_bar[s], st + kTileABytes, kx, y, kEvictFirst);
+                    tma_load_2d(&tm[2], &full_bar[s], st + 2 * kTileABytes, kx, 0, kEvictLast);
+                    tma_load_2d(&tm[3], &full_bar[s], st + 2 * kTileABytes + Cfg::kTileBBytes, kx, 0, kEvictLast);
+                }
+            }
+        }
+    } else {
+        int it = 0;
+        for (int u = blockIdx.x; u < P.n_units; u += gridDim.x) {
+            const GroupUnit w = group_unit(P.cls, P.n_classes, u);
+            float acc[N / 2];
+#pragma unroll
+            for (int j = 0; j < N / 2; ++j) acc[j] = 0.f;
+            mma_kblocks<N, Cfg::kStages, Cfg::kStageBytes>(acc, smem, full_bar, empty_bar, it, it + (w.kb1 - w.kb0));
+            it += w.kb1 - w.kb0;
+            const GroupClass& c = P.cls[w.cls];
+            const int64_t row0 = (int64_t)w.m_tile * kBlockM + 64 * (warp >> 2);
+            float* out = c.partial + ((int64_t)w.slice * c.m) * N;
+#pragma unroll
+            for (int j = 0; j < N / 2; j += 2) {
+                const int64_t row = row0 + frag_row(warp, lane, j);
+                if (row < c.m) *reinterpret_cast<float2*>(out + row * N + frag_col(lane, j)) = make_float2(acc[j], acc[j + 1]);
+            }
+        }
+    }
+}
+
+// The classes of a group for the given splits, sorted longest first (stable: problem order, full slices before last slices).
+// partial may be null (planning only).  Returns the number of classes.
+static int group_classes(int np, const int64_t* m, const int64_t* n, const int64_t* k, const int* split, float* const* partial,
+                         GroupClass* cls) {
+    int nc = 0;
+    for (int p = 0; p < np; ++p) {
+        const int total_kb = (int)((k[p] + kBlockK - 1) / kBlockK);
+        const int per = (total_kb + split[p] - 1) / split[p];
+        const int last = total_kb - per * (split[p] - 1);
+        const int m_tiles = (int)((m[p] + kBlockM - 1) / kBlockM);
+        GroupClass c{partial ? partial[p] : nullptr, p, (int)m[p], m_tiles, per, 0, 0, 0, per};
+        const int full = (last == per) ? split[p] : split[p] - 1;
+        if (full > 0) { c.n_units = full * m_tiles; cls[nc++] = c; }
+        if (full < split[p]) { c.s0 = full; c.len = last; c.n_units = m_tiles; cls[nc++] = c; }
+    }
+    for (int i = 1; i < nc; ++i)   // insertion sort, stable
+        for (int j = i; j > 0 && cls[j].len > cls[j - 1].len; --j) { GroupClass t = cls[j]; cls[j] = cls[j - 1]; cls[j - 1] = t; }
+    int u0 = 0;
+    for (int i = 0; i < nc; ++i) { cls[i].u0 = u0; u0 += cls[i].n_units; }
+    (void)n;
+    return nc;
+}
+
+static int group_grid(int n_units, int n, int max_ctas) {
+    int g = kNumSMs * ctas_per_sm(n);
+    if (max_ctas > 0 && max_ctas < g) g = max_ctas;
+    return n_units < g ? n_units : g;
+}
+
+// Estimated time of the round-robin schedule, in k-blocks of the busiest CTA.  A unit also costs its partial tile
+// (128 x N fp32): written here and read again by the epilogue, about two k-blocks of A (128 x 64 bf16 hi + lo) per 64 of N.
+static int64_t group_cost(const GroupClass* cls, int nc, int grid, int n) {
+    const int64_t unit_cost = 2 * n / 64;
+    int64_t load[kNumSMs * 2] = {0};
+    for (int i = 0; i < nc; ++i) {
+        const int64_t per_cta = cls[i].n_units / grid, rem = cls[i].n_units % grid, first = cls[i].u0 % grid;
+        const int64_t c = cls[i].len + unit_cost;
+        for (int b = 0; b < grid; ++b) {
+            const int64_t off = (b - first + grid) % grid;
+            load[b] += c * (per_cta + (off < rem ? 1 : 0));
+        }
+    }
+    int64_t worst = 0;
+    for (int b = 0; b < grid; ++b) worst = load[b] > worst ? load[b] : worst;
+    return worst;
+}
+
 }  // namespace mmssl
 
 using namespace mmssl;
@@ -158,4 +303,135 @@ extern "C" int mmssl_gemm_bf16x3(const uint16_t* a_hi, const uint16_t* a_lo, int
     if (n == 64) return launch_gemm<64>(ah, al, bh, bl, partial, m, k, split_k, st);
     if (n == 128) return launch_gemm<128>(ah, al, bh, bl, partial, m, k, split_k, st);
     return launch_gemm<256>(ah, al, bh, bl, partial, m, k, split_k, st);
+}
+
+namespace mmssl {
+
+// Splits of a group: the plan of the estimated shortest round-robin schedule (group_cost).  The single-problem plans
+// (choose_split) are tried first and kept unless another plan is strictly shorter, so a group whose problems already
+// balance computes bitwise the partials of mmssl_gemm_bf16x3.  Every slice stays within kMaxChainKb k-blocks.
+static void group_plan(int np, const int64_t* m, const int64_t* n, const int64_t* k, int max_ctas, int* split) {
+    GroupClass cls[2 * kGroupMax];
+    int cand[kGroupMax][kMaxChainKb], n_cand[kGroupMax];
+    for (int p = 0; p < np; ++p) {
+        split[p] = choose_split(m[p], n[p], k[p]);
+        const int total_kb = (int)((k[p] + kBlockK - 1) / kBlockK);
+        n_cand[p] = 0;
+        for (int per = total_kb < kMaxChainKb ? total_kb : kMaxChainKb; per >= 1; --per) {   // fewest slices first
+            const int s = (total_kb + per - 1) / per;
+            if (s > kMaxSplit) break;
+            if (n_cand[p] == 0 || cand[p][n_cand[p] - 1] != s) cand[p][n_cand[p]++] = s;
+        }
+    }
+    auto cost = [&](const int* sp) {
+        const int nc = group_classes(np, m, n, k, sp, nullptr, cls);
+        const int units = cls[nc - 1].u0 + cls[nc - 1].n_units;
+        return group_cost(cls, nc, group_grid(units, (int)n[0], max_ctas), (int)n[0]);
+    };
+    int64_t best = cost(split);
+    int trial[kGroupMax];
+    for (int i = 0; i < n_cand[0]; ++i)
+        for (int j = 0; j < (np > 1 ? n_cand[1] : 1); ++j) {
+            trial[0] = cand[0][i];
+            if (np > 1) trial[1] = cand[1][j];
+            const int64_t c = cost(trial);
+            if (c < best) {
+                best = c;
+                for (int p = 0; p < np; ++p) split[p] = trial[p];
+            }
+        }
+}
+
+static int group_check_shapes(int np, const int64_t* m, const int64_t* n, const int64_t* k) {
+    MMSSL_REQUIRE(np >= 1 && np <= kGroupMax, "a group holds one or two problems");
+    for (int p = 0; p < np; ++p) {
+        MMSSL_REQUIRE(n[p] == 64 || n[p] == 128 || n[p] == 256, "n (embedding width) must be 64, 128 or 256");
+        MMSSL_REQUIRE(n[p] == n[0], "the problems of a group must have the same n");
+        MMSSL_REQUIRE(m[p] >= 1 && k[p] >= 1 && m[p] < (1ll << 31) && k[p] < (1ll << 31), "bad m / k");
+    }
+    return 0;
+}
+
+template <int N>
+static int launch_group(const GroupParams& prm, int grid, cudaStream_t st) {
+    using Cfg = GemmCfg<N>;
+    static bool attr_done = false;
+    if (!attr_done) {
+        MMSSL_CUDA(cudaFuncSetAttribute(gemm_bf16x3_group_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+        attr_done = true;
+    }
+    gemm_bf16x3_group_kernel<N><<<grid, kThreads, Cfg::kSmemBytes, st>>>(prm);
+    MMSSL_LAUNCH_OK();
+    return 0;
+}
+
+}  // namespace mmssl
+
+extern "C" int64_t mmssl_gemm_bf16x3_group_plan(int n_problems, const int64_t* mnk, int max_ctas, int* split_out,
+                                                int64_t* floats_out, int32_t* units_out, int64_t units_cap) {
+    int64_t m[kGroupMax], n[kGroupMax], k[kGroupMax];
+    if (n_problems < 1 || n_problems > kGroupMax || mnk == nullptr) {
+        fail(__func__, "a group holds one or two problems");
+        return -1;
+    }
+    for (int p = 0; p < n_problems; ++p) { m[p] = mnk[3 * p]; n[p] = mnk[3 * p + 1]; k[p] = mnk[3 * p + 2]; }
+    if (group_check_shapes(n_problems, m, n, k)) return -1;
+    int split[kGroupMax];
+    group_plan(n_problems, m, n, k, max_ctas, split);
+    GroupClass cls[2 * kGroupMax];
+    const int nc = group_classes(n_problems, m, n, k, split, nullptr, cls);
+    const int64_t units = cls[nc - 1].u0 + cls[nc - 1].n_units;
+    for (int p = 0; p < n_problems; ++p) {
+        if (split_out) split_out[p] = split[p];
+        if (floats_out) floats_out[p] = (int64_t)split[p] * m[p] * n[p];
+    }
+    if (units_out)
+        for (int64_t u = 0; u < units && u < units_cap; ++u) {
+            const GroupUnit w = group_unit(cls, nc, (int)u);
+            units_out[4 * u] = cls[w.cls].prob;
+            units_out[4 * u + 1] = w.m_tile;
+            units_out[4 * u + 2] = w.kb0;
+            units_out[4 * u + 3] = w.kb1;
+        }
+    return units;
+}
+
+extern "C" int mmssl_gemm_bf16x3_group(int n_problems, const mmssl_gemm_problem_t* probs, int max_ctas, void* stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    MMSSL_REQUIRE(n_problems >= 1 && n_problems <= kGroupMax && probs != nullptr, "a group holds one or two problems");
+    MMSSL_REQUIRE(max_ctas >= 0, "max_ctas must be >= 0 (0 = one resident wave)");
+    int64_t m[kGroupMax], n[kGroupMax], k[kGroupMax];
+    int split[kGroupMax];
+    float* partial[kGroupMax];
+    GroupParams prm;
+    memset(&prm, 0, sizeof(prm));
+    for (int p = 0; p < n_problems; ++p) {
+        const mmssl_gemm_problem_t& q = probs[p];
+        m[p] = q.m; n[p] = q.n; k[p] = q.k; split[p] = q.split_k; partial[p] = q.partial;
+    }
+    if (int rc = group_check_shapes(n_problems, m, n, k)) return rc;
+    for (int p = 0; p < n_problems; ++p) {
+        const mmssl_gemm_problem_t& q = probs[p];
+        MMSSL_REQUIRE(q.lda % 8 == 0 && q.ldb % 8 == 0 && q.lda >= q.k && q.ldb >= q.k,
+                      "lda/ldb must be >= k and multiples of 8 (16-byte TMA strides)");
+        MMSSL_REQUIRE(aligned16(q.a_hi) && aligned16(q.a_lo) && aligned16(q.b_hi) && aligned16(q.b_lo) && aligned16(q.partial),
+                      "alignment");
+        const int total_kb = (int)((q.k + kBlockK - 1) / kBlockK);
+        MMSSL_REQUIRE(q.split_k >= 1 && q.split_k <= total_kb, "split_k out of range");
+        const int per = (total_kb + q.split_k - 1) / q.split_k;
+        MMSSL_REQUIRE((int64_t)per * (q.split_k - 1) < total_kb, "split_k leaves an empty K slice (use mmssl_gemm_bf16x3_group_plan)");
+        MMSSL_REQUIRE(per <= kMaxChainKb, "a K slice is longer than kMaxChainKb k-blocks (use mmssl_gemm_bf16x3_group_plan)");
+        MMSSL_REQUIRE((int64_t)q.split_k * ((q.m + kBlockM - 1) / kBlockM) < (1ll << 30), "too many units");
+        if (int rc = make_map(&prm.maps[p][0], q.a_hi, q.m, q.lda, kBlockM)) return rc;
+        if (int rc = make_map(&prm.maps[p][1], q.a_lo, q.m, q.lda, kBlockM)) return rc;
+        if (int rc = make_map(&prm.maps[p][2], q.b_hi, q.n, q.ldb, (int)q.n)) return rc;
+        if (int rc = make_map(&prm.maps[p][3], q.b_lo, q.n, q.ldb, (int)q.n)) return rc;
+    }
+    prm.n_problems = n_problems;
+    prm.n_classes = group_classes(n_problems, m, n, k, split, partial, prm.cls);
+    prm.n_units = prm.cls[prm.n_classes - 1].u0 + prm.cls[prm.n_classes - 1].n_units;
+    const int grid = group_grid(prm.n_units, (int)n[0], max_ctas);
+    if (n[0] == 64) return launch_group<64>(prm, grid, st);
+    if (n[0] == 128) return launch_group<128>(prm, grid, st);
+    return launch_group<256>(prm, grid, st);
 }

@@ -6,7 +6,7 @@ and its hand-derived backward as an explicit sequence of library kernels.  No au
 drives it directly (fused with the loss kernels and AdamW, CUDA-graph captured).
 
 Launch inventory of one forward (K GCN layers, modality graphs aliasing ui/iu as at step 0,
-main.py:68-69):  2 projections x (split, GEMM, epilogue) + 2 two-RHS SpMM (image|text batched)
+main.py:68-69):  2 W splits + 1 grouped projection GEMM + 2 epilogues + 2 two-RHS SpMM (image|text batched)
 + 2 id SpMM + Wsum + 2 fused id-fusion kernels + 2K SpMM (softmax / layer-sum fused) + 2 combine kernels,
 scheduled on three streams (see ``Engine.two_streams``).
 """
@@ -77,6 +77,10 @@ class Engine:
         self.d, self.K, self.H = embed_size, n_layers, head_num
         self.id_rate, self.cat_rate = id_cat_rate, model_cat_rate
         self.proj_impl = proj_impl
+        # Grid of the grouped projection GEMM: one CTA per SM (132 on the H100 SXM) rather than the full two-per-SM wave.  The
+        # persistent CTAs would otherwise hold every slot while the id / GCN branch runs beside them; measured on an H100 at
+        # 700 W, 132 CTAs gave the shorter Baby and Sports steps (DESIGN section 6).  MMSSL_PROJ_MAX_CTAS overrides it (0 = full wave).
+        self.proj_max_ctas = int(os.environ.get("MMSSL_PROJ_MAX_CTAS", 132))
         self._tile_id: Dict[Tuple, torch.Tensor] = {}
         # The modality branch (projection -> A_ui [Xv|Xt] -> A_iu [Uv|Ut]) and the id/GCN branch are
         # independent until the final combine (and again after combine-backward), so they run on two
@@ -168,35 +172,58 @@ class Engine:
         return torch.empty(*shape, dtype=torch.float32, device=dev)
 
     # ------------------------------------------------------------------ projection
-    def _project(self, w, b, fs: FeatureStore, mask, y, y_pre=None):
-        I, d, D = fs.n_items, self.d, fs.dim
-        if self.proj_impl == "tc":
+    def _project(self, P, feats, masks, ys):
+        """X = F W^T + b, then the dropout mask, for image and text (Models.py:173-174).  Tensor cores: both GEMMs in ONE
+        grouped persistent launch (the feature streams of 118 + 30 MB at Baby share one balanced wave), then the two
+        split-K epilogues."""
+        d = self.d
+        ws, bs = (P[P_WV], P[P_WT]), (P[P_BV], P[P_BT])
+        if self.proj_impl != "tc":
+            self._fork2(ys[0].device, lambda: self._project_simt(ws[0], bs[0], feats[0], masks[0], ys[0]),
+                        lambda: self._project_simt(ws[1], bs[1], feats[1], masks[1], ys[1]))
+            return
+        splits, floats = ops.gemm_bf16x3_group_plan([(fs.n_items, d, fs.dim) for fs in feats], self.proj_max_ctas)
+        parts = self._new(sum(floats), dev=ys[0].device).split(floats)
+        probs = []
+        for w, fs, sk, part in zip(ws, feats, splits, parts):
             w_hi, w_lo = ops.split_bf16(w)
-            floats, sk = ops.gemm_bf16x3_plan(I, d, D)
-            part = self._new(floats, dev=y.device)
-            ops.gemm_bf16x3(fs.hi, fs.lo, w_hi, w_lo, I, d, D, sk, part)
-        else:
-            if fs.fp32 is None:
-                raise RuntimeError("proj_impl='simt' needs the fp32 features (keep_fp32=True)")
-            sk = 1
-            part = self._new(I, d, dev=y.device)
-            ops.sgemm(fs.fp32, w, part, trans_b=True)
-        ops.proj_epilogue(part, sk, I, d, b, mask, y, y_pre)
+            probs.append((fs.hi, fs.lo, w_hi, w_lo, fs.n_items, d, fs.dim, sk, part))
+        ops.gemm_bf16x3_group(probs, self.proj_max_ctas)
+        for b, fs, sk, part, mask, y in zip(bs, feats, splits, parts, masks, ys):
+            ops.proj_epilogue(part, sk, fs.n_items, d, b, mask, y)
 
-    def _project_bwd(self, gx, mask, fs: FeatureStore, dw, db):
-        """dW[d,D] = (gx*mask)^T F ; db = colsum(gx*mask)."""
-        I, d, D = fs.n_items, self.d, fs.dim
-        if self.proj_impl == "tc":
-            g_hi, g_lo = ops.split_bf16_t(gx, mask, ldo=fs.t_hi.shape[1], colsum=db)   # [d, ceil8(I)]; db from the same pass
-            floats, sk = ops.gemm_bf16x3_plan(D, d, I)
-            part = self._new(floats, dev=gx.device)
-            ops.gemm_bf16x3(fs.t_hi, fs.t_lo, g_hi, g_lo, D, d, I, sk, part)
-            ops.wgrad_epilogue(part, sk, D, d, dw)
-        else:
-            gm = self._new(I, d, dev=gx.device)
-            ops.mul_mask(gx, mask, gm)
-            ops.sgemm(gm, fs.fp32, dw, trans_a=True)
-            ops.colsum(gx, mask, db)
+    def _project_simt(self, w, b, fs: FeatureStore, mask, y):
+        I, d = fs.n_items, self.d
+        if fs.fp32 is None:
+            raise RuntimeError("proj_impl='simt' needs the fp32 features (keep_fp32=True)")
+        part = self._new(I, d, dev=y.device)
+        ops.sgemm(fs.fp32, w, part, trans_b=True)
+        ops.proj_epilogue(part, 1, I, d, b, mask, y)
+
+    def _project_bwd(self, gxs, masks, feats, dws, dbs):
+        """dW[d,D] = (gx*mask)^T F ; db = colsum(gx*mask), for image and text.  Tensor cores: the operand splits (db from
+        the same pass), both weight-gradient GEMMs in ONE grouped persistent launch, then the two epilogues."""
+        d = self.d
+        if self.proj_impl != "tc":
+            self._fork2(gxs[0].device, lambda: self._project_bwd_simt(gxs[0], masks[0], feats[0], dws[0], dbs[0]),
+                        lambda: self._project_bwd_simt(gxs[1], masks[1], feats[1], dws[1], dbs[1]))
+            return
+        splits, floats = ops.gemm_bf16x3_group_plan([(fs.dim, d, fs.n_items) for fs in feats], self.proj_max_ctas)
+        parts = self._new(sum(floats), dev=gxs[0].device).split(floats)
+        probs = []
+        for gx, mask, fs, db, sk, part in zip(gxs, masks, feats, dbs, splits, parts):
+            g_hi, g_lo = ops.split_bf16_t(gx, mask, ldo=fs.t_hi.shape[1], colsum=db)   # [d, ceil8(I)]
+            probs.append((fs.t_hi, fs.t_lo, g_hi, g_lo, fs.dim, d, fs.n_items, sk, part))
+        ops.gemm_bf16x3_group(probs, self.proj_max_ctas)
+        for fs, sk, part, dw in zip(feats, splits, parts, dws):
+            ops.wgrad_epilogue(part, sk, fs.dim, d, dw)
+
+    def _project_bwd_simt(self, gx, mask, fs: FeatureStore, dw, db):
+        I, d = fs.n_items, self.d
+        gm = self._new(I, d, dev=gx.device)
+        ops.mul_mask(gx, mask, gm)
+        ops.sgemm(gm, fs.fp32, dw, trans_a=True)
+        ops.colsum(gx, mask, db)
 
     # ------------------------------------------------------------------ forward
     def forward(self, P: Dict[str, torch.Tensor], feats: Tuple[FeatureStore, FeatureStore],
@@ -222,9 +249,7 @@ class Engine:
                 side_pre()
             m = masks() if callable(masks) else masks
             resolved[0] = m
-            # the two projections are independent HBM streams (118 + 30 MB at Baby): side by side on two streams
-            self._fork2(dev, lambda: self._project(P[P_WV], P[P_BV], feats[0], m[0] if m else None, xv),    # Models.py:173
-                        lambda: self._project(P[P_WT], P[P_BT], feats[1], m[1] if m else None, xt))         # Models.py:174
+            self._project(P, feats, m if m else (None, None), (xv, xt))                 # Models.py:173-174
             self._spmm(g_ui, "fwd", [xv, xt], "i", [uv, ut])                        # :177,182
             self._spmm(g_iu, "fwd", [uv, ut], "u", [iv, it])                        # :178,183
 
@@ -346,8 +371,8 @@ class Engine:
             gX2 = self._new(I, 2 * d, dev=dev)
             self._spmm(g_ui, "bwd", [gU2[:, :d], gU2[:, d:]], "u", [gX2[:, :d], gX2[:, d:]])
             m = st.masks
-            self._fork2(dev, lambda: self._project_bwd(gX2[:, :d], m[0] if m else None, feats[0], w_slots[0], w_slots[1]),
-                        lambda: self._project_bwd(gX2[:, d:], m[1] if m else None, feats[1], w_slots[2], w_slots[3]))
+            self._project_bwd((gX2[:, :d], gX2[:, d:]), m if m else (None, None), feats, (w_slots[0], w_slots[2]),
+                              (w_slots[1], w_slots[3]))
             return gX2
 
         if side is not main:

@@ -442,3 +442,35 @@ def gemm_bf16x3(a_hi, a_lo, b_hi, b_lo, m, n, k, split_k, partial):
     _lib.check(lib.mmssl_gemm_bf16x3(ptr(a_hi), ptr(a_lo), a_hi.stride(0), ptr(b_hi), ptr(b_lo), b_hi.stride(0), m, n, k,
                                      split_k, ptr(partial), stream()))
     return partial
+
+
+def gemm_bf16x3_group_plan(shapes, max_ctas=0, units=False):
+    """Plan of one grouped launch over 1-2 problems, shapes = [(m, n, k), ...] with the same n.
+    Returns (splits, floats) per problem; with units=True also the [n_units, 4] int32 list (problem, m_tile, kb_begin,
+    kb_end) in the order the CTAs walk it."""
+    lib = _lib_()
+    np_ = len(shapes)
+    mnk = (C.c_int64 * (3 * np_))(*[int(v) for s in shapes for v in s])
+    sk = (C.c_int32 * np_)()
+    fl = (C.c_int64 * np_)()
+    n_units = lib.mmssl_gemm_bf16x3_group_plan(np_, mnk, int(max_ctas), sk, fl, None, 0)
+    if n_units < 0:
+        _lib.check(1)
+    splits, floats = [int(v) for v in sk], [int(v) for v in fl]
+    if not units:
+        return splits, floats
+    buf = torch.zeros(n_units, 4, dtype=torch.int32, device="cpu")
+    lib.mmssl_gemm_bf16x3_group_plan(np_, mnk, int(max_ctas), sk, fl, C.c_void_p(buf.data_ptr()), n_units)
+    return splits, floats, buf
+
+
+def gemm_bf16x3_group(problems, max_ctas=0):
+    """One persistent launch for 1-2 problems (a_hi, a_lo, b_hi, b_lo, m, n, k, split_k, partial): each partial[s][m][n]
+    as gemm_bf16x3 with the same split_k computes it."""
+    lib = _lib_()
+    arr = (_lib.GemmProblem * len(problems))()
+    for q, (a_hi, a_lo, b_hi, b_lo, m, n, k, sk, part) in zip(arr, problems):
+        q.a_hi, q.a_lo, q.lda = a_hi.data_ptr(), a_lo.data_ptr(), a_hi.stride(0)
+        q.b_hi, q.b_lo, q.ldb = b_hi.data_ptr(), b_lo.data_ptr(), b_hi.stride(0)
+        q.m, q.n, q.k, q.split_k, q.partial = m, n, k, sk, part.data_ptr()
+    _lib.check(lib.mmssl_gemm_bf16x3_group(len(problems), arr, int(max_ctas), stream()))
