@@ -270,15 +270,28 @@ int mmssl_dp_fused_adamw_dev(const float* p_local, float* p_mc, const float* g_m
                              float eps, float weight_decay, void* stream);
 
 /* ------------------------------------------------------------------ GPU triple sampler (SURVEY 8f "next" #1)
- * Semantics of Data.sample (utility/load_data.py:153-191): `batch` (<= 1024) distinct users with >= 1
+ * Semantics of Data.sample (utility/load_data.py:153-191): `batch` distinct users with >= 1
  * training item (with replacement only if batch > n_exist), one uniform positive from the user's CSR row
  * (indptr/indices int64, rows sorted), one uniform negative rejected against the row.  Counter-based RNG
  * keyed by (seed, step); step is read from *step_dev when non-NULL (graph replay), else step_host.
- * claim[n_exist] is a work table initialised once with mmssl_sampler_init and left clean by every launch. */
+ * mmssl_sample_triples: batch <= 1024, one CTA; claim[n_exist] is a work table initialised once with
+ * mmssl_sampler_init and left clean by every launch. */
 int mmssl_sampler_init(int32_t* claim, int64_t n_exist, void* stream);
 int mmssl_sample_triples(const int64_t* indptr, const int64_t* indices, const int64_t* exist, int64_t n_exist,
                          int64_t n_items, int batch, uint64_t seed, const int32_t* step_dev, int32_t step_host,
                          int32_t* claim, int64_t* users, int64_t* pos, int64_t* neg, void* stream);
+/* Any batch size: the users are the slots of the `batch` smallest keys (hash32(seed, step, slot) << 32 | slot), found by a
+ * multi-CTA radix select over all n_exist slots (O(n_exist) per call) and returned in key order; batch == n_exist is a
+ * permutation.  batch > n_exist draws with replacement.  Depends only on (seed, step, batch).  The workspace
+ * (mmssl_sampler_workspace_bytes, 0 when batch > n_exist) is zero-filled once before its first use and left so by every
+ * call; no allocation and no host synchronisation per call, so the launch is CUDA-graph capturable.  The workspace holds
+ * the select's counters between kernels: calls that share one workspace must not overlap (one stream, or one graph
+ * replay at a time); concurrent callers use one workspace each. */
+int64_t mmssl_sampler_workspace_bytes(int64_t n_exist, int batch);
+int mmssl_sample_triples_multi(const int64_t* indptr, const int64_t* indices, const int64_t* exist, int64_t n_exist,
+                               int64_t n_items, int batch, uint64_t seed, const int32_t* step_dev, int32_t step_host,
+                               void* workspace, int64_t workspace_bytes, int64_t* users, int64_t* pos, int64_t* neg,
+                               void* stream);
 
 /* ------------------------------------------------------------------ evaluation (SURVEY 8f "next" #3)
  * Trainer.test -> test_torch / test_one_user (main.py:301-306, utility/batch_test.py:21-36, :83-169) and

@@ -106,6 +106,9 @@ _SIGS = {
     "mmssl_dp_fused_adamw_dev": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_f32, c_vp, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp]),
     "mmssl_sampler_init": (C.c_int, [c_vp, c_i64, c_vp]),
     "mmssl_sample_triples": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i32, C.c_uint64, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "mmssl_sampler_workspace_bytes": (c_i64, [c_i64, c_i32]),
+    "mmssl_sample_triples_multi": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i32, C.c_uint64, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp,
+                                             c_vp]),
     "mmssl_eval_rank": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, C.POINTER(c_i32), c_i32,
                                   c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "mmssl_eval_full_stage": (C.c_int, []),
@@ -157,13 +160,15 @@ _SIGS = {
 _lib = None
 
 # kernels launched by one call of each entry point (for bench.py's gpu_launches claim)
+# (mmssl_sample_triples_multi: an approximate count -- 8 select passes + compaction + draw + CUB's radix sort, whose
+# launch count depends on the batch and the key width; 1 when the batch exceeds the eligible users)
 KERNELS_PER_CALL = {
     "mmssl_csr_from_coo": 6, "mmssl_csr_row_normalize": 1, "mmssl_spmm_plan": 8, "mmssl_spmm_csr_f32": 1, "mmssl_spmm_hot_f32": 1, "mmssl_spmm_bulk_plan": 9, "mmssl_spmm_bulk_f32": 1, "mmssl_reduce_rows_epilogue": 1, "mmssl_sgemm": 1,
     "mmssl_id_fuse_fwd": 1, "mmssl_id_fuse_bwd": 1, "mmssl_wsum": 1, "mmssl_id_fuse2_fwd": 1, "mmssl_id_fuse2_bwd": 1,
     "mmssl_dwcat_reduce": 1, "mmssl_combine_fwd": 1, "mmssl_combine_bwd": 1, "mmssl_softmax_bwd": 1,
     "mmssl_axpby": 1, "mmssl_mul_mask": 1, "mmssl_sumsq": 1, "mmssl_bpr": 1, "mmssl_infonce_prepare": 1,
     "mmssl_infonce_stats": 2, "mmssl_infonce_grad": 1, "mmssl_infonce_scatter": 1, "mmssl_infonce_stats_tc": 4, "mmssl_infonce_forward_tc": 3, "mmssl_infonce_grad_tc": 1, "mmssl_loss_assemble": 1,
-    "mmssl_step_tick": 1, "mmssl_dp_fused_adamw": 1, "mmssl_dp_fused_adamw_dev": 1, "mmssl_sampler_init": 1, "mmssl_sample_triples": 1, "mmssl_adamw": 1, "mmssl_split_bf16": 1, "mmssl_split_bf16_t": 1, "mmssl_split_bf16_t_colsum": 1, "mmssl_gemm_bf16x3": 1, "mmssl_gemm_bf16x3_group": 1, "mmssl_gemm_bf16x3_wide": 1,
+    "mmssl_step_tick": 1, "mmssl_dp_fused_adamw": 1, "mmssl_dp_fused_adamw_dev": 1, "mmssl_sampler_init": 1, "mmssl_sample_triples": 1, "mmssl_sample_triples_multi": 20, "mmssl_adamw": 1, "mmssl_split_bf16": 1, "mmssl_split_bf16_t": 1, "mmssl_split_bf16_t_colsum": 1, "mmssl_gemm_bf16x3": 1, "mmssl_gemm_bf16x3_group": 1, "mmssl_gemm_bf16x3_wide": 1,
     "mmssl_proj_epilogue": 1, "mmssl_wgrad_epilogue": 1, "mmssl_colsum": 1,
     "mmssl_eval_rank": 1, "mmssl_eval_rank_full": 1, "mmssl_eval_rank_wide": 1, "mmssl_eval_reduce": 1,
     "mmssl_gan_bn_fwd": 1, "mmssl_gan_bn_bwd": 1, "mmssl_gan_gp_rev_bn": 1, "mmssl_gan_bn_fwd_rev": 1, "mmssl_gan_colsum": 1,

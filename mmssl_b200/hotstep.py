@@ -56,6 +56,8 @@ class HotStep:
         self.batch = batch
         self.optimizer_step = optimizer_step
         self.sampler = sampler          # optional sampler.DeviceTripleSampler: batches are drawn on the device
+        if sampler is not None:
+            sampler.reserve(batch)      # workspace of the multi-CTA path (batch > 1024) before any capture
         self.grad_sync = None           # optional callable run between backward and AdamW (data-parallel all-reduce)
         # optional callable(outs, st) -> (g_Iv, g_It, g_Uv, g_Ut): extra output gradients of the forward, e.g. the
         # G_rate * G_lossf term of the full step (main.py:414-420); runs after the loss kernels, before the backward
