@@ -13,6 +13,8 @@
 //   multimem.ld_reduce.add.v4.f32 / multimem.st.v4.f32         over multicast groups registered by the test (cuemu_mc_register):
 //                                                               several ranks' replicas in one process
 //   fences, prefetch.tensormap, griddepcontrol.wait             no-ops
+//   ld.global[.nc] / st.global with L1:: / L2::cache_hint       plain loads and stores (.b32, .f32, .v4.f32, incl. the predicated
+//                                                               @q / @!q pair of common.cuh:ldg4_l1_hot_cold); hints are not modelled
 // What the model asserts on the way: 1024-byte aligned swizzled tiles, transaction bytes that add up, barrier phases, the
 // descriptor fields the kernels are supposed to encode, the accumulator fragment size of the instruction shape.  A kernel that
 // passes here and shares tc_common.cuh's descriptor / swizzle code with proj_tc.cu (tests/test_emu_tensor_core.py) differs
@@ -271,7 +273,26 @@ void ptx_op(const char* text, void** outs, const int* out_sizes, int n_out, cons
         for (uint8_t* r : g.replicas) memcpy(r + off, v, 16);
         return;
     }
-    (void)n_in;
+    if ((has("ld.global") || has("st.global")) && (has("L2::cache_hint") || has("L1::"))) {
+        // cache-hinted loads / stores (common.cuh): plain memory accesses here, the hints only steer residency.  A load
+        // writes n_out consecutive 32-bit values from in[0]; the predicated @q / @!q pair of ldg4_l1_hot_cold loads the same
+        // address into the same registers on both branches, so it is one load.  A store takes the address and its values,
+        // then the policy word.
+        const bool st = has("st.global");
+        const int nv = st ? n_in - 2 : n_out;
+        if (nv != 1 && nv != 4) fail("cache-hinted access: only .b32 / .f32 and .v4.f32 are modelled");
+        if (in[0] % (4u * (unsigned)nv)) fail("cache-hinted access: misaligned address");
+        if (st) {
+            uint32_t v[4];
+            for (int k = 0; k < nv; ++k) v[k] = (uint32_t)in[1 + k];
+            memcpy(reinterpret_cast<void*>((uintptr_t)in[0]), v, 4 * nv);
+        } else {
+            uint32_t v[4];
+            memcpy(v, reinterpret_cast<const void*>((uintptr_t)in[0]), 4 * nv);
+            for (int k = 0; k < nv; ++k) out32(outs, out_sizes, k, v[k]);
+        }
+        return;
+    }
     std::string m = std::string("inline PTX is not emulated: ") + text;
     fail(m.c_str());
 }

@@ -3,6 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "common.cuh"
+using namespace mmssl;
+
 __global__ void st_shuffles(int* out) {          // out[5][blockDim.x]
     const int t = threadIdx.x, lane = t & 31, n = blockDim.x;
     int v = t * 3 + 1;
@@ -75,6 +78,18 @@ __global__ void st_ptx(int* out) {
     if (out[1] == 7) asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %1, %1, %1};" ::"l"(out), "f"(1.f) : "memory");
 }
 
+// the cache-hinted accesses of common.cuh: out[0..3] <- stream loads, out[4..7] <- L2-policy / L1 hot / cold loads of a
+// (hot and cold alike), out[8] <- b32 stream load, out[9] <- f32 stream load; out[12..15] <- st4_stream of out[0..3] + 1
+__global__ void st_cache_hints(const float* a, float* out) {
+    const float4 v = ldg4_stream(a), w = ld4_stream(a + 4);
+    const float4 l2 = ldg4_l2(a + 8, kL2EvictLast), hot = ldg4_l1_hot_cold(a + 12, 1, kL2EvictLast), cold = ldg4_l1_hot_cold(a + 16, 0, 0);
+    out[0] = v.x; out[1] = v.y; out[2] = w.z; out[3] = w.w;
+    out[4] = l2.x; out[5] = hot.y; out[6] = cold.z; out[7] = cold.w;
+    out[8] = (float)ldg_i32_stream(reinterpret_cast<const int*>(a + 20));
+    out[9] = ldg_f32_stream(a + 21);
+    st4_stream(out + 12, make_float4(out[0] + 1.f, out[1] + 1.f, out[2] + 1.f, out[3] + 1.f));
+}
+
 extern "C" int cuemu_st_run(int which, void* a, void* b, void* c, int n, int block, int grid) {
     cudaGetLastError();
     switch (which) {
@@ -86,6 +101,7 @@ extern "C" int cuemu_st_run(int which, void* a, void* b, void* c, int n, int blo
         case 6: st_bad_mask<<<1, 64>>>((int*)a); break;
         case 7: st_ptx<<<1, 1>>>((int*)a); break;
         case 8: st_shuffles<<<1, 2048>>>((int*)a); break;       // invalid configuration
+        case 9: st_cache_hints<<<1, 1>>>((const float*)a, (float*)b); break;
         default: return -1;
     }
     return (int)cudaPeekAtLastError();

@@ -92,3 +92,16 @@ def test_deadlock_ptx_and_bad_configuration_are_reported():
     rc, msg = _run(8, np.zeros(5 * 2048, np.int32))
     assert rc != 0 and "invalid launch configuration" in msg
     assert _run(0, np.zeros((5, 32), np.int32), block=32)[0] == 0     # the error does not stick to later launches
+
+
+def test_cache_hinted_loads_and_stores():
+    """common.cuh's L1 / L2-hinted accesses (SpMM impl bits 7 and 8) are plain loads and stores in the model, both branches of
+    the predicated hot / cold load included."""
+    harness.set_order("fwd")
+    a = np.arange(1, 25, dtype=np.float32)
+    a.view(np.int32)[20] = 12345
+    out = np.zeros(16, np.float32)
+    rc, msg = _run(9, a, out)
+    assert rc == 0, msg
+    assert out[:10].tolist() == [1, 2, 7, 8, 9, 14, 19, 20, 12345, 22]
+    assert out[12:].tolist() == [2, 3, 8, 9]
