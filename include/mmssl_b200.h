@@ -26,6 +26,10 @@ int mmssl_abi_version(void);
 const char* mmssl_last_error(void);
 /* 0 if the current device is compute capability 9.x (H100); fails loudly otherwise. */
 int mmssl_device_check(void);
+/* 1 if the row kernels (SpMM, row ops, losses) and the projection are built for embedding width d: 32, 64, 96, 128, 192
+ * or 256.  The tensor-core InfoNCE (d in {64, 128}), the fused id fusion (d in {64, 128}) and the hot-row / staged-gather
+ * SpMM variants (d in {64, 128, 256}) cover fewer widths; mmssl_spmm_csr_f32 at d = 32, 96, 192 takes impl 0, 4 or 16. */
+int mmssl_embed_width_supported(int d);
 
 /* ------------------------------------------------------------------ graph preparation
  * Replaces the per-call coalesce + COO->CSR conversion ATen performs inside torch.sparse.mm

@@ -42,6 +42,7 @@ _SIGS = {
     "mmssl_abi_version": (C.c_int, []),
     "mmssl_last_error": (C.c_char_p, []),
     "mmssl_device_check": (C.c_int, []),
+    "mmssl_embed_width_supported": (C.c_int, [c_i32]),
     "mmssl_csr_workspace_bytes": (c_i64, [c_i64, c_i64]),
     "mmssl_csr_from_coo": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "mmssl_csr_row_normalize": (C.c_int, [c_vp, c_i64, c_vp, c_vp]),

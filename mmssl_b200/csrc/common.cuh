@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <type_traits>
 namespace mmssl {
 
 // ---- error reporting (thread-local message, C-ABI functions return non-zero on failure) ----
@@ -146,6 +147,30 @@ __device__ __forceinline__ float group_max(float v, unsigned mask) {
     return v;
 }
 __device__ __forceinline__ float warp_sum(float v) { return group_sum<32>(v, 0xffffffffu); }
+
+// ---- embedding widths ----
+// The row kernels (SpMM, row ops, losses) lay a row of d floats over a group of G consecutive lanes, G a power of two from 8
+// to 32 (group_sum), each lane holding C float4 per right-hand side at columns 4 lane + 4 G c: d = 4 G C.  These six widths
+// are the ones the library is built for; kernel dispatch and host-side sizes derived from G both come from this rule.
+struct WidthShape { int g, c; };
+constexpr WidthShape width_shape(int d) {
+    return d == 32 ? WidthShape{8, 1} : d == 64 ? WidthShape{16, 1} : d == 96 ? WidthShape{8, 3}
+         : d == 128 ? WidthShape{32, 1} : d == 192 ? WidthShape{16, 3} : d == 256 ? WidthShape{32, 2} : WidthShape{0, 0};
+}
+constexpr bool width_supported(int d) { return width_shape(d).g != 0; }
+int fail_width(const char* where, int d);   // "<where>: embedding width <d> is not supported (...)"
+
+// f(integral_constant G, integral_constant C) for one of the six widths, an error naming the width otherwise.
+template <typename F>
+static inline int dispatch_width(int d, F&& f, const char* where = "embedding width") {
+#define MMSSL_WIDTH_CASE(D) \
+    case D: return f(std::integral_constant<int, width_shape(D).g>(), std::integral_constant<int, width_shape(D).c>());
+    switch (d) {
+        MMSSL_WIDTH_CASE(32) MMSSL_WIDTH_CASE(64) MMSSL_WIDTH_CASE(96) MMSSL_WIDTH_CASE(128) MMSSL_WIDTH_CASE(192) MMSSL_WIDTH_CASE(256)
+    }
+#undef MMSSL_WIDTH_CASE
+    return fail_width(where, d);
+}
 
 // Block-wide sum for blockDim.x <= 1024 (result valid in thread 0).
 __device__ __forceinline__ float block_sum(float v, float* smem32) {

@@ -5,8 +5,6 @@
 // losses are read from device scalars so nothing syncs with the host).
 #include <cuda_bf16.h>
 
-#include <type_traits>
-
 #include "common.cuh"
 #include "../../include/mmssl_b200.h"
 
@@ -146,13 +144,16 @@ constexpr int NS = NT + 4;      // smem row stride: float4-aligned rows, conflic
 // 256 threads = 16 (ty) x 16 (tx).  Shared-memory traffic is what bounds these tiles, so every operand
 // is read with 128-bit loads along its contiguous axis (4 reduction steps per load).
 
+// RAGGED: d is not a multiple of NT (d = 32, 96, 192), so the last chunk of the d axis sticks out past d and is zero-filled;
+// off, the chunks tile d exactly and the instance compiles to the code it had before the flag existed.
+template <bool RAGGED>
 __device__ __forceinline__ void load_tile(float* sm, const float* __restrict__ src, int64_t row0, int64_t n, int d,
                                           int c0) {
-    // sm[r][k] = src[(row0+r)*d + c0 + k], r,k < 64 (zero beyond n)
+    // sm[r][k] = src[(row0+r)*d + c0 + k], r,k < 64 (zero beyond n, and beyond d when RAGGED)
     for (int e = threadIdx.x; e < NT * (NT / 4); e += 256) {
         const int r = e / (NT / 4), k4 = (e % (NT / 4)) * 4;
         float4 v = f4zero();
-        if (row0 + r < n) v = ld4(src + (row0 + r) * (int64_t)d + c0 + k4);
+        if (row0 + r < n && (!RAGGED || c0 + k4 < d)) v = ld4(src + (row0 + r) * (int64_t)d + c0 + k4);
         *reinterpret_cast<float4*>(sm + r * NS + k4) = v;
     }
 }
@@ -207,6 +208,7 @@ __device__ __forceinline__ void tile_tn(float (&acc)[4][4], const float* Q, cons
 }
 
 // stats layout: [diagR n][diagB n][loss n][unused n][partR ntj*n][partB ntj*n]
+template <bool RAGGED>
 __global__ void __launch_bounds__(256) nce_stats_kernel(const float* __restrict__ a, const float* __restrict__ b,
                                                         int64_t n, int d, float inv_tau, float* __restrict__ stats) {
     pdl_wait();
@@ -216,9 +218,9 @@ __global__ void __launch_bounds__(256) nce_stats_kernel(const float* __restrict_
     const int64_t i0 = blockIdx.x * (int64_t)NT, j0 = blockIdx.y * (int64_t)NT;
     float sr[4][4] = {}, sb[4][4] = {};
     for (int c0 = 0; c0 < d; c0 += NT) {
-        load_tile(Ai, a, i0, n, d, c0);
-        load_tile(Aj, a, j0, n, d, c0);
-        load_tile(Bj, b, j0, n, d, c0);
+        load_tile<RAGGED>(Ai, a, i0, n, d, c0);
+        load_tile<RAGGED>(Aj, a, j0, n, d, c0);
+        load_tile<RAGGED>(Bj, b, j0, n, d, c0);
         __syncthreads();
         tile_nt(sr, Ai, Aj, ty, tx);
         tile_nt(sb, Ai, Bj, ty, tx);
@@ -286,6 +288,7 @@ __global__ void __launch_bounds__(256) nce_finalize_kernel(int64_t n, int64_t nt
     if (threadIdx.x == 0) loss_part[blockIdx.x] = tot;
 }
 
+template <bool RAGGED>
 __global__ void __launch_bounds__(256) nce_grad_kernel(const float* __restrict__ a, const float* __restrict__ b,
                                                        int64_t n, int d, float inv_tau, const float* __restrict__ coef,
                                                        float* __restrict__ ga, float* __restrict__ gb) {
@@ -297,9 +300,9 @@ __global__ void __launch_bounds__(256) nce_grad_kernel(const float* __restrict__
     const int64_t i0 = blockIdx.x * (int64_t)NT, j0 = blockIdx.y * (int64_t)NT;
     float sr[4][4] = {}, sb[4][4] = {};
     for (int c0 = 0; c0 < d; c0 += NT) {
-        load_tile(Ai, a, i0, n, d, c0);
-        load_tile(Aj, a, j0, n, d, c0);
-        load_tile(Bj, b, j0, n, d, c0);
+        load_tile<RAGGED>(Ai, a, i0, n, d, c0);
+        load_tile<RAGGED>(Aj, a, j0, n, d, c0);
+        load_tile<RAGGED>(Bj, b, j0, n, d, c0);
         __syncthreads();
         tile_nt(sr, Ai, Aj, ty, tx);
         tile_nt(sb, Ai, Bj, ty, tx);
@@ -328,9 +331,9 @@ __global__ void __launch_bounds__(256) nce_grad_kernel(const float* __restrict__
     __syncthreads();
     for (int c0 = 0; c0 < d; c0 += NT) {
         if (d > NT) {   // tiles of the first chunk pass are gone when d has several chunks
-            load_tile(Ai, a, i0, n, d, c0);
-            load_tile(Aj, a, j0, n, d, c0);
-            load_tile(Bj, b, j0, n, d, c0);
+            load_tile<RAGGED>(Ai, a, i0, n, d, c0);
+            load_tile<RAGGED>(Aj, a, j0, n, d, c0);
+            load_tile<RAGGED>(Bj, b, j0, n, d, c0);
             __syncthreads();
         }
         float g1[4][4] = {}, g2[4][4] = {};
@@ -343,6 +346,7 @@ __global__ void __launch_bounds__(256) nce_grad_kernel(const float* __restrict__
 #pragma unroll
             for (int jj = 0; jj < 4; ++jj) {
                 const int c = c0 + tx * 4 + jj;
+                if (RAGGED && c >= d) continue;
                 if (i < n) atomicAdd(ga + i * d + c, g1[ii][jj]);
                 if (j < n) atomicAdd(gb + j * d + c, g2[ii][jj]);
             }
@@ -448,20 +452,12 @@ __global__ void __launch_bounds__(1024) loss_assemble_kernel(const float* bpr_pa
     }
 }
 
-template <typename F>
-static int dispatch_d(int d, F&& f) {
-    if (d == 64) return f(std::integral_constant<int, 16>(), std::integral_constant<int, 1>());
-    if (d == 128) return f(std::integral_constant<int, 32>(), std::integral_constant<int, 1>());
-    if (d == 256) return f(std::integral_constant<int, 32>(), std::integral_constant<int, 2>());
-    return fail("loss", "embedding width must be 64, 128 or 256");
-}
-
 }  // namespace mmssl
 
 using namespace mmssl;
 #define GV(x) decltype(x)::value
 
-extern "C" int64_t mmssl_bpr_blocks(int64_t batch, int d) { return (batch * (d == 64 ? 16 : 32) + 255) / 256; }
+extern "C" int64_t mmssl_bpr_blocks(int64_t batch, int d) { return (batch * width_shape(d).g + 255) / 256; }
 
 extern "C" int mmssl_bpr(const float* uf, int64_t ldu, const float* itf, int64_t ldi, const float* itf_neg, int64_t ldin,
                          const int64_t* users, const int64_t* pos, const int64_t* neg, int64_t batch, int d, int mode,
@@ -474,13 +470,13 @@ extern "C" int mmssl_bpr(const float* uf, int64_t ldu, const float* itf, int64_t
     MMSSL_REQUIRE(!(mode & 2) || (g_uf && g_pos && g_neg && aligned16(g_uf) && aligned16(g_pos) && aligned16(g_neg) &&
                                   ldgu % 4 == 0 && ldgp % 4 == 0 && ldgn % 4 == 0), "mode bit 1 needs gradient buffers");
     if (batch == 0) return 0;
-    return dispatch_d(d, [&](auto G, auto C) {
+    return dispatch_width(d, [&](auto G, auto C) {
         const unsigned blocks = (unsigned)mmssl_bpr_blocks(batch, d);
         MMSSL_CUDA_LAUNCH((bpr_kernel<GV(G), GV(C)>), dim3(blocks), dim3(256), 0, st, uf, ldu, itf, ldi, itf_neg, ldin, users, pos, neg, batch, mode,
                                                          reg_coef, g_mf, g_emb, part, g_uf, ldgu, g_pos, ldgp, g_neg, ldgn);
         MMSSL_LAUNCH_OK();
         return 0;
-    });
+    }, __func__);
 }
 
 extern "C" int mmssl_infonce_prepare(const float* z1, int64_t ldz1, const float* z2, int64_t ldz2, const int64_t* idx,
@@ -489,24 +485,25 @@ extern "C" int mmssl_infonce_prepare(const float* z1, int64_t ldz1, const float*
     cudaStream_t st = (cudaStream_t)stream_;
     MMSSL_REQUIRE(aligned16(z1) && aligned16(z2) && ldz1 % 4 == 0 && ldz2 % 4 == 0 && aligned16(a) && aligned16(b), "alignment");
     if (n == 0) return 0;
-    return dispatch_d(d, [&](auto G, auto C) {
+    return dispatch_width(d, [&](auto G, auto C) {
         const unsigned blocks = (unsigned)((n * GV(G) + 255) / 256);
         MMSSL_CUDA_LAUNCH((nce_prepare_kernel<GV(G), GV(C)>), dim3(blocks), dim3(256), 0, st, z1, ldz1, z2, ldz2, idx, n, a, b, na, nb, ga, gb,
                           (uint16_t*)nullptr, (uint16_t*)nullptr, (uint16_t*)nullptr, (uint16_t*)nullptr);
         MMSSL_LAUNCH_OK();
         return 0;
-    });
+    }, __func__);
 }
 
 // [diagR n][diagB n][loss n][unused n][partR ntj*n][partB ntj*n]; ntj <= ceil(n / 64) + 1 (the tensor-core path uses 2 per 128-tile)
 extern "C" int64_t mmssl_infonce_stats_floats(int64_t n) { return 4 * n + 2 * n * ((n + NT - 1) / NT + 1); }
 extern "C" int64_t mmssl_infonce_loss_blocks(int64_t n) { return (n + 255) / 256; }
 
+template <bool RAGGED>
 static int nce_smem_attr() {
     static bool done = false;
     if (done) return 0;
-    MMSSL_CUDA(cudaFuncSetAttribute(nce_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * NT * NS * 4));
-    MMSSL_CUDA(cudaFuncSetAttribute(nce_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * NT * NS * 4));
+    MMSSL_CUDA(cudaFuncSetAttribute(nce_stats_kernel<RAGGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * NT * NS * 4));
+    MMSSL_CUDA(cudaFuncSetAttribute(nce_grad_kernel<RAGGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 5 * NT * NS * 4));
     done = true;
     return 0;
 }
@@ -514,12 +511,14 @@ static int nce_smem_attr() {
 extern "C" int mmssl_infonce_stats(const float* a, const float* b, int64_t n, int d, float inv_tau, float* stats,
                                    float* coef, const float* g_loss, float* loss_part, void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
-    MMSSL_REQUIRE(d % NT == 0, "d must be a multiple of 64");
+    MMSSL_REQUIRE(d > 0 && d % 4 == 0, "d must be a positive multiple of 4");
     if (n == 0) return 0;
-    if (int rc = nce_smem_attr()) return rc;
+    const bool ragged = d % NT != 0;
+    if (int rc = ragged ? nce_smem_attr<true>() : nce_smem_attr<false>()) return rc;
     const unsigned nt = (unsigned)((n + NT - 1) / NT);
     MMSSL_REQUIRE(nt <= 65535, "batch too large for one InfoNCE call");
-    MMSSL_CUDA_LAUNCH((nce_stats_kernel), dim3(dim3(nt, nt)), dim3(256), 3 * NT * NS * 4, st, a, b, n, d, inv_tau, stats);
+    if (ragged) MMSSL_CUDA_LAUNCH((nce_stats_kernel<true>), dim3(dim3(nt, nt)), dim3(256), 3 * NT * NS * 4, st, a, b, n, d, inv_tau, stats);
+    else MMSSL_CUDA_LAUNCH((nce_stats_kernel<false>), dim3(dim3(nt, nt)), dim3(256), 3 * NT * NS * 4, st, a, b, n, d, inv_tau, stats);
     MMSSL_LAUNCH_OK();
     MMSSL_CUDA_LAUNCH((nce_finalize_kernel), dim3((unsigned)mmssl_infonce_loss_blocks(n)), dim3(256), 0, st, n, nt, stats, coef, g_loss, loss_part);
     MMSSL_LAUNCH_OK();
@@ -533,13 +532,13 @@ int nce_prepare_split_launch(const float* z1, int64_t ldz1, const float* z2, int
                              float* b, float* na, float* nb, uint16_t* a_hi, uint16_t* a_lo, uint16_t* b_hi, uint16_t* b_lo, cudaStream_t st) {
     MMSSL_REQUIRE(aligned16(z1) && aligned16(z2) && ldz1 % 4 == 0 && ldz2 % 4 == 0 && aligned16(a) && aligned16(b), "alignment");
     if (n == 0) return 0;
-    return dispatch_d(d, [&](auto G, auto C) {
+    return dispatch_width(d, [&](auto G, auto C) {
         const unsigned blocks = (unsigned)((n * GV(G) + 255) / 256);
         MMSSL_CUDA_LAUNCH((nce_prepare_kernel<GV(G), GV(C)>), dim3(blocks), dim3(256), 0, st, z1, ldz1, z2, ldz2, idx, n, a, b, na, nb,
                           (float*)nullptr, (float*)nullptr, a_hi, a_lo, b_hi, b_lo);
         MMSSL_LAUNCH_OK();
         return 0;
-    });
+    }, __func__);
 }
 
 // loss rows + backward coefficients from the row sums of `ntj` column tiles (used by the tensor-core path, loss_tc.cu)
@@ -553,12 +552,14 @@ int nce_finalize_launch(int64_t n, int64_t ntj, float* stats, float* coef, const
 extern "C" int mmssl_infonce_grad(const float* a, const float* b, int64_t n, int d, float inv_tau, const float* coef,
                                   float* ga, float* gb, void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
-    MMSSL_REQUIRE(d % NT == 0, "d must be a multiple of 64");
+    MMSSL_REQUIRE(d > 0 && d % 4 == 0, "d must be a positive multiple of 4");
     if (n == 0) return 0;
-    if (int rc = nce_smem_attr()) return rc;
+    const bool ragged = d % NT != 0;
+    if (int rc = ragged ? nce_smem_attr<true>() : nce_smem_attr<false>()) return rc;
     const unsigned nt = (unsigned)((n + NT - 1) / NT);
     MMSSL_REQUIRE(nt <= 65535, "batch too large for one InfoNCE call");
-    MMSSL_CUDA_LAUNCH((nce_grad_kernel), dim3(dim3(nt, nt)), dim3(256), 5 * NT * NS * 4, st, a, b, n, d, inv_tau, coef, ga, gb);
+    if (ragged) MMSSL_CUDA_LAUNCH((nce_grad_kernel<true>), dim3(dim3(nt, nt)), dim3(256), 5 * NT * NS * 4, st, a, b, n, d, inv_tau, coef, ga, gb);
+    else MMSSL_CUDA_LAUNCH((nce_grad_kernel<false>), dim3(dim3(nt, nt)), dim3(256), 5 * NT * NS * 4, st, a, b, n, d, inv_tau, coef, ga, gb);
     MMSSL_LAUNCH_OK();
     return 0;
 }
@@ -569,12 +570,12 @@ extern "C" int mmssl_infonce_scatter(const float* ga, const float* gb, const flo
     cudaStream_t st = (cudaStream_t)stream_;
     MMSSL_REQUIRE((g_z1 == nullptr || (aligned16(g_z1) && ldg1 % 4 == 0)) && (g_z2 == nullptr || (aligned16(g_z2) && ldg2 % 4 == 0)), "alignment");
     if (n == 0) return 0;
-    return dispatch_d(d, [&](auto G, auto C) {
+    return dispatch_width(d, [&](auto G, auto C) {
         const unsigned blocks = (unsigned)((n * GV(G) + 255) / 256);
         MMSSL_CUDA_LAUNCH((nce_scatter_kernel<GV(G), GV(C)>), dim3(blocks), dim3(256), 0, st, ga, gb, a, b, na, nb, idx, n, g_z1, ldg1, g_z2, ldg2);
         MMSSL_LAUNCH_OK();
         return 0;
-    });
+    }, __func__);
 }
 
 extern "C" int mmssl_loss_assemble(const float* bpr_part, int64_t n_bpr_blocks, int64_t batch, float reg_coef,

@@ -21,17 +21,20 @@
 
 namespace mmssl {
 
+// N = 32 and 64: two CTAs are co-resident per SM (2 stages each: 160 / 192 KB of loads in flight),
+// so one CTA's prologue / epilogue overlaps the other's main loop.
+static constexpr int ctas_per_sm(int64_t n) { return n <= 64 ? 2 : 1; }
+static bool proj_width_ok(int64_t n) { return n == 32 || n == 64 || n == 96 || n == 128 || n == 192 || n == 256; }
+
 template <int N>
 struct GemmCfg {
     static constexpr int kTileBBytes = N * kBlockK * 2;
-    static constexpr int kStageBytes = 2 * kTileABytes + 2 * kTileBBytes;
-    // N = 64: two CTAs are co-resident per SM (2 stages each = the same 192 KB of loads in flight),
-    // so one CTA's prologue / epilogue overlaps the other's main loop.
-    static constexpr int kCtasPerSm = (N == 64) ? 2 : 1;
-    static constexpr int kStages = (N == 64) ? 2 : (N == 128 ? 3 : 2);
+    static constexpr int kStageBytes = 2 * kTileABytes + 2 * kTileBBytes;   // 32 KB of A (hi + lo) + N * 256 B of B
+    static constexpr int kCtasPerSm = ctas_per_sm(N);
+    // 2 x 40 / 48 KB per CTA at N = 32 / 64; 3 x 56 / 64 KB at N = 96 / 128; 2 x 80 / 128 KB at N = 192 / 256
+    static constexpr int kStages = (N <= 64) ? 2 : (N <= 128 ? 3 : 2);
     static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
-static constexpr int ctas_per_sm(int64_t n) { return n == 64 ? 2 : 1; }   // GemmCfg<n>::kCtasPerSm
 constexpr int kGroupMax = 2;                                                // problems of one grouped launch (image, text)
 
 template <int N>
@@ -96,7 +99,7 @@ static int choose_split(int64_t m, int64_t n, int64_t k) {
     // (e.g. 56 M-tiles x 4 slices = 224 of 264 slots) instead of leaving a nearly empty tail wave.
     const int64_t total_kb = (k + kBlockK - 1) / kBlockK;
     const int64_t m_tiles = (m + kBlockM - 1) / kBlockM;
-    const int64_t slots = (int64_t)kNumSMs * (n == 64 ? 2 : 1);
+    const int64_t slots = (int64_t)kNumSMs * ctas_per_sm(n);
     int64_t split = slots / m_tiles;
     // accuracy: the tensor core's fp32 accumulate is not round-to-nearest and its error grows linearly with the number of MMAs
     // chained into one accumulator (gemm_wide.cu; the weight gradient at 200k items with 347 k-blocks per slice was 1e-4 off).  A slice is therefore at most kMaxChainKb k-blocks long; the slices are summed in fp32 by the epilogue.
@@ -285,7 +288,7 @@ extern "C" int mmssl_gemm_bf16x3(const uint16_t* a_hi, const uint16_t* a_lo, int
                                  const uint16_t* b_lo, int64_t ldb, int64_t m, int64_t n, int64_t k, int split_k,
                                  float* partial, void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
-    MMSSL_REQUIRE(n == 64 || n == 128 || n == 256, "n (embedding width) must be 64, 128 or 256");
+    MMSSL_REQUIRE(proj_width_ok(n), "n (embedding width) must be 32, 64, 96, 128, 192 or 256");
     MMSSL_REQUIRE(m >= 1 && k >= 1 && m < (1ll << 31) && k < (1ll << 31), "bad m / k");
     MMSSL_REQUIRE(lda % 8 == 0 && ldb % 8 == 0 && lda >= k && ldb >= k, "lda/ldb must be >= k and multiples of 8 (16-byte TMA strides)");
     MMSSL_REQUIRE(aligned16(a_hi) && aligned16(a_lo) && aligned16(b_hi) && aligned16(b_lo) && aligned16(partial), "alignment");
@@ -300,9 +303,14 @@ extern "C" int mmssl_gemm_bf16x3(const uint16_t* a_hi, const uint16_t* a_lo, int
     if (int rc = make_map(&al, a_lo, m, lda, kBlockM)) return rc;
     if (int rc = make_map(&bh, b_hi, n, ldb, (int)n)) return rc;
     if (int rc = make_map(&bl, b_lo, n, ldb, (int)n)) return rc;
-    if (n == 64) return launch_gemm<64>(ah, al, bh, bl, partial, m, k, split_k, st);
-    if (n == 128) return launch_gemm<128>(ah, al, bh, bl, partial, m, k, split_k, st);
-    return launch_gemm<256>(ah, al, bh, bl, partial, m, k, split_k, st);
+    switch (n) {
+        case 32: return launch_gemm<32>(ah, al, bh, bl, partial, m, k, split_k, st);
+        case 64: return launch_gemm<64>(ah, al, bh, bl, partial, m, k, split_k, st);
+        case 96: return launch_gemm<96>(ah, al, bh, bl, partial, m, k, split_k, st);
+        case 128: return launch_gemm<128>(ah, al, bh, bl, partial, m, k, split_k, st);
+        case 192: return launch_gemm<192>(ah, al, bh, bl, partial, m, k, split_k, st);
+        default: return launch_gemm<256>(ah, al, bh, bl, partial, m, k, split_k, st);
+    }
 }
 
 namespace mmssl {
@@ -345,7 +353,7 @@ static void group_plan(int np, const int64_t* m, const int64_t* n, const int64_t
 static int group_check_shapes(int np, const int64_t* m, const int64_t* n, const int64_t* k) {
     MMSSL_REQUIRE(np >= 1 && np <= kGroupMax, "a group holds one or two problems");
     for (int p = 0; p < np; ++p) {
-        MMSSL_REQUIRE(n[p] == 64 || n[p] == 128 || n[p] == 256, "n (embedding width) must be 64, 128 or 256");
+        MMSSL_REQUIRE(proj_width_ok(n[p]), "n (embedding width) must be 32, 64, 96, 128, 192 or 256");
         MMSSL_REQUIRE(n[p] == n[0], "the problems of a group must have the same n");
         MMSSL_REQUIRE(m[p] >= 1 && k[p] >= 1 && m[p] < (1ll << 31) && k[p] < (1ll << 31), "bad m / k");
     }
@@ -431,7 +439,12 @@ extern "C" int mmssl_gemm_bf16x3_group(int n_problems, const mmssl_gemm_problem_
     prm.n_classes = group_classes(n_problems, m, n, k, split, partial, prm.cls);
     prm.n_units = prm.cls[prm.n_classes - 1].u0 + prm.cls[prm.n_classes - 1].n_units;
     const int grid = group_grid(prm.n_units, (int)n[0], max_ctas);
-    if (n[0] == 64) return launch_group<64>(prm, grid, st);
-    if (n[0] == 128) return launch_group<128>(prm, grid, st);
-    return launch_group<256>(prm, grid, st);
+    switch (n[0]) {
+        case 32: return launch_group<32>(prm, grid, st);
+        case 64: return launch_group<64>(prm, grid, st);
+        case 96: return launch_group<96>(prm, grid, st);
+        case 128: return launch_group<128>(prm, grid, st);
+        case 192: return launch_group<192>(prm, grid, st);
+        default: return launch_group<256>(prm, grid, st);
+    }
 }

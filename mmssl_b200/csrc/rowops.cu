@@ -1,12 +1,10 @@
 // Row-wise fused glue of MMSSL.forward / backward: everything between the SpMMs that is not a GEMM.
-// One lane group (16 lanes for d=64, 32 otherwise) owns one row, float4 per lane, shuffle reductions;
+// One lane group (width_shape in common.cuh: 8 to 32 lanes) owns one row, float4 per lane, shuffle reductions;
 // all kernels are HBM/L2-bound streaming passes.
 //   id_fuse      Models.py:196-197   u0 = E + id_cat_rate * normalize(z)
 //   combine      Models.py:213-218   uf = mean_k(u_k) + model_cat_rate*(normalize(Uv)+normalize(Ut))
 //                                    (+ the sums of squares main.py:252-257 needs, for free)
 //   softmax_bwd  backward of Models.py:203-204
-#include <type_traits>
-
 #include "common.cuh"
 #include "../../include/mmssl_b200.h"
 
@@ -293,13 +291,6 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ g
     }
 }
 
-template <typename F>
-static int dispatch_d(int d, F&& f) {
-    if (d == 64) return f(std::integral_constant<int, 16>(), std::integral_constant<int, 1>());
-    if (d == 128) return f(std::integral_constant<int, 32>(), std::integral_constant<int, 1>());
-    if (d == 256) return f(std::integral_constant<int, 32>(), std::integral_constant<int, 2>());
-    return fail("rowops", "embedding width must be 64, 128 or 256");
-}
 static inline unsigned row_blocks(int64_t n, int g) { return (unsigned)((n * g + 255) / 256); }
 
 }  // namespace mmssl
@@ -312,11 +303,11 @@ extern "C" int mmssl_id_fuse_fwd(const float* z, int64_t ldz, const float* e, in
     cudaStream_t st = (cudaStream_t)stream_;
     MMSSL_REQUIRE(ROW_ALIGN_OK(z, ldz) && ROW_ALIGN_OK(e, lde) && ROW_ALIGN_OK(out, ldo) && aligned16(zn), "alignment");
     if (n == 0) return 0;
-    return dispatch_d(d, [&](auto G, auto C) {
+    return dispatch_width(d, [&](auto G, auto C) {
         MMSSL_CUDA_LAUNCH((id_fuse_fwd_kernel<decltype(G)::value, decltype(C)::value>), dim3(row_blocks(n, decltype(G)::value)), dim3(256), 0, st, z, ldz, e, lde, n, rate, out, ldo, zn, nrm);
         MMSSL_LAUNCH_OK();
         return 0;
-    });
+    }, __func__);
 }
 
 extern "C" int mmssl_id_fuse_bwd(const float* g, int64_t ldg, const float* zn, const float* nrm, int64_t n, int d,
@@ -324,14 +315,14 @@ extern "C" int mmssl_id_fuse_bwd(const float* g, int64_t ldg, const float* zn, c
     cudaStream_t st = (cudaStream_t)stream_;
     MMSSL_REQUIRE(ROW_ALIGN_OK(g, ldg) && ROW_ALIGN_OK(dz, lddz) && aligned16(zn), "alignment");
     if (n == 0) return 0;
-    return dispatch_d(d, [&](auto G, auto C) {
+    return dispatch_width(d, [&](auto G, auto C) {
         MMSSL_CUDA_LAUNCH((id_fuse_bwd_kernel<decltype(G)::value, decltype(C)::value>), dim3(row_blocks(n, decltype(G)::value)), dim3(256), 0, st, g, ldg, zn, nrm, n, rate, dz, lddz);
         MMSSL_LAUNCH_OK();
         return 0;
-    });
+    }, __func__);
 }
 
-extern "C" int64_t mmssl_combine_partials(int64_t n, int d) { return (n * (d == 64 ? 16 : 32) + 255) / 256; }
+extern "C" int64_t mmssl_combine_partials(int64_t n, int d) { return (n * width_shape(d).g + 255) / 256; }
 
 extern "C" int mmssl_combine_fwd(const float* s, int64_t lds, const float* a, int64_t lda, const float* b, int64_t ldb,
                                  int64_t n, int d, float inv_layers, float rate, float* out, int64_t ldo,
@@ -340,12 +331,12 @@ extern "C" int mmssl_combine_fwd(const float* s, int64_t lds, const float* a, in
     MMSSL_REQUIRE(ROW_ALIGN_OK(s, lds) && ROW_ALIGN_OK(a, lda) && ROW_ALIGN_OK(b, ldb) && ROW_ALIGN_OK(out, ldo), "alignment");
     MMSSL_REQUIRE(sumsq_partials == nullptr || n_partials >= mmssl_combine_partials(n, d), "sumsq_partials too small");
     if (n == 0) return 0;
-    return dispatch_d(d, [&](auto G, auto C) {
+    return dispatch_width(d, [&](auto G, auto C) {
         MMSSL_CUDA_LAUNCH((combine_fwd_kernel<decltype(G)::value, decltype(C)::value>), dim3(row_blocks(n, decltype(G)::value)), dim3(256), 0, st, s, lds, a, lda, b, ldb, n, inv_layers,
                                                                                    rate, out, ldo, sumsq_partials);
         MMSSL_LAUNCH_OK();
         return 0;
-    });
+    }, __func__);
 }
 
 extern "C" int mmssl_combine_bwd(const float* g, int64_t ldg, const float* a, int64_t lda, const float* b, int64_t ldb,
@@ -357,13 +348,13 @@ extern "C" int mmssl_combine_bwd(const float* g, int64_t ldg, const float* a, in
                       ROW_ALIGN_OK(gb, ldgb), "alignment");
     MMSSL_REQUIRE((ga_ext == nullptr || ROW_ALIGN_OK(ga_ext, ldgae)) && (gb_ext == nullptr || ROW_ALIGN_OK(gb_ext, ldgbe)), "alignment");
     if (n == 0) return 0;
-    return dispatch_d(d, [&](auto G, auto C) {
+    return dispatch_width(d, [&](auto G, auto C) {
         MMSSL_CUDA_LAUNCH((combine_bwd_kernel<decltype(G)::value, decltype(C)::value>), dim3(row_blocks(n, decltype(G)::value)), dim3(256), 0, st, g, ldg, a, lda, b, ldb, ga_ext, ldgae,
                                                                                    gb_ext, ldgbe, n, rate, reg_coef, ga,
                                                                                    ldga, gb, ldgb);
         MMSSL_LAUNCH_OK();
         return 0;
-    });
+    }, __func__);
 }
 
 extern "C" int mmssl_softmax_bwd(const float* y, int64_t ldy, const float* g, int64_t ldg, int64_t n, int d, float alpha,
@@ -371,11 +362,11 @@ extern "C" int mmssl_softmax_bwd(const float* y, int64_t ldy, const float* g, in
     cudaStream_t st = (cudaStream_t)stream_;
     MMSSL_REQUIRE(ROW_ALIGN_OK(y, ldy) && ROW_ALIGN_OK(g, ldg) && ROW_ALIGN_OK(t, ldt), "alignment");
     if (n == 0) return 0;
-    return dispatch_d(d, [&](auto G, auto C) {
+    return dispatch_width(d, [&](auto G, auto C) {
         MMSSL_CUDA_LAUNCH((softmax_bwd_kernel<decltype(G)::value, decltype(C)::value>), dim3(row_blocks(n, decltype(G)::value)), dim3(256), 0, st, y, ldy, g, ldg, n, alpha, t, ldt);
         MMSSL_LAUNCH_OK();
         return 0;
-    });
+    }, __func__);
 }
 
 extern "C" int mmssl_axpby(const float* x, int64_t ldx, int64_t n, int d, float alpha, const float* alpha_dev, float beta,
@@ -415,12 +406,13 @@ extern "C" int mmssl_sumsq(const float* x, int64_t ldx, int64_t n, int d, float*
 extern "C" int mmssl_colsum(const float* g, int64_t ldg, const float* mask, int64_t ldm, int64_t rows, int n, float* out,
                             int accumulate, void* stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
-    MMSSL_REQUIRE(n >= 1 && n <= 256 && 256 % n == 0, "n must divide 256");
+    MMSSL_REQUIRE(n >= 1 && n <= 256, "n must be 1..256");
     if (!accumulate) MMSSL_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * n, st));
     if (rows == 0) return 0;
     const int rows_per_block = 64;
     const unsigned blocks = (unsigned)((rows + rows_per_block - 1) / rows_per_block);
-    MMSSL_CUDA_LAUNCH((colsum_kernel), dim3(blocks), dim3(256), 256 * sizeof(float), st, g, ldg, mask, ldm, rows, n, rows_per_block, out);
+    const unsigned threads = (256 / n) * n;      // a whole number of rows per pass (256 when n divides it; 192 at n = 96)
+    MMSSL_CUDA_LAUNCH((colsum_kernel), dim3(blocks), dim3(threads), 256 * sizeof(float), st, g, ldg, mask, ldm, rows, n, rows_per_block, out);
     MMSSL_LAUNCH_OK();
     return 0;
 }

@@ -176,7 +176,7 @@ extern "C" int mmssl_reduce_rows_epilogue(int64_t n_rows, int d, int nrhs, const
     SpmmParams p;
     if (int rc = fill_spmm_params(p, &a, d, nrhs, rhs, epilogue, alpha, s_mode, nullptr, 0)) return rc;
     cudaStream_t st = (cudaStream_t)stream_;
-    if (d == 64) return launch_reduce_rows<16, 1>(p, nrhs, n_rows, multicast, st);
-    if (d == 128) return launch_reduce_rows<32, 1>(p, nrhs, n_rows, multicast, st);
-    return launch_reduce_rows<32, 2>(p, nrhs, n_rows, multicast, st);
+    return dispatch_width(d, [&](auto G, auto C) {
+        return launch_reduce_rows<decltype(G)::value, decltype(C)::value>(p, nrhs, n_rows, multicast, st);
+    }, __func__);
 }

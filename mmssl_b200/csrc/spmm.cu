@@ -4,7 +4,7 @@
 //
 // Design (sparse gather: latency bound on small graphs, L2-gather / resident-row-walk bound on
 // large ones -- DESIGN.md section 6; no tensor cores):
-//  * one lane *group* (16 lanes for d=64, 32 lanes for d>=128) owns one work item = one row or one
+//  * one lane *group* (width_shape, common.cuh: 8 lanes for d = 32 / 96, 16 for 64 / 192, 32 for 128 / 256) owns one work item = one row or one
 //    fixed-length segment of a long row (plan built by mmssl_spmm_plan); every lane owns one
 //    float4 column slice per right-hand side, so a neighbour row is fetched with one coalesced
 //    128-bit load per lane (256 B .. 1 KB contiguous per neighbour).
@@ -373,11 +373,17 @@ static int launch_spmm(const SpmmParams& p, cudaStream_t stream, int T, int impl
     }
 }
 
+// impl 4 (128-thread blocks, small graphs) and impl 16 (register-capped, 6 blocks / SM, from 2^21 non-zeros): what impl 0 selects
+template <int G, int C, int R>
+static int launch_spmm_auto(const SpmmParams& p, cudaStream_t stream, int T, int impl) {
+    return (impl & 16) ? launch_spmm_v<G, C, R, 1, 6>(p, stream, T) : launch_spmm_v<G, C, R, 1, 1>(p, stream, T);
+}
+
 int fill_spmm_params(SpmmParams& p, const mmssl_csr_t* a, int d, int nrhs, const mmssl_spmm_rhs_t* rhs, int epilogue,
                      float alpha, int s_mode, float* partials, int64_t partials_floats) {
     MMSSL_REQUIRE(a != nullptr && rhs != nullptr, "null argument");
     MMSSL_REQUIRE(nrhs >= 1 && nrhs <= kMaxRhs, "nrhs must be 1..3");
-    MMSSL_REQUIRE(d == 64 || d == 128 || d == 256, "embedding width must be 64, 128 or 256");
+    if (!width_supported(d)) return fail_width(__func__, d);
     MMSSL_REQUIRE(epilogue >= MMSSL_EPI_NONE && epilogue <= MMSSL_EPI_SOFTMAX_BWD, "bad epilogue");
     MMSSL_REQUIRE(s_mode >= 0 && s_mode <= 2, "bad s_mode");
     MMSSL_REQUIRE(a->n_items >= 0 && a->items != nullptr, "missing work plan");
@@ -450,6 +456,20 @@ extern "C" int mmssl_spmm_csr_f32(const mmssl_csr_t* a, int d, int nrhs, const m
     if (d == 64 && (impl & 2)) { MMSSL_SPMM_CASE(8, 2) }
     if (d == 64) { MMSSL_SPMM_CASE(16, 1) }
     if (d == 128) { MMSSL_SPMM_CASE(32, 1) }
-    MMSSL_SPMM_CASE(32, 2)
+    if (d == 256) { MMSSL_SPMM_CASE(32, 2) }
 #undef MMSSL_SPMM_CASE
+    // d = 32, 96, 192: only the two launch shapes the automatic policy picks are built (each variant is one more set of
+    // template instances per width)
+    if (impl != 4 && impl != 16) {
+        snprintf(last_error_buffer(), 512, "mmssl_spmm_csr_f32: embedding width %d takes impl 0, 4 or 16 only (got %d)", d, impl);
+        return 1;
+    }
+    return dispatch_width(d, [&](auto G_, auto C_) {
+        constexpr int G = decltype(G_)::value, C = decltype(C_)::value;
+        switch (nrhs) {
+            case 1: return launch_spmm_auto<G, C, 1>(p, stream, T, impl);
+            case 2: return launch_spmm_auto<G, C, 2>(p, stream, T, impl);
+            default: return launch_spmm_auto<G, C, 3>(p, stream, T, impl);
+        }
+    }, "mmssl_spmm_csr_f32");
 }

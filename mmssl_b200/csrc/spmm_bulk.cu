@@ -443,6 +443,7 @@ extern "C" int mmssl_spmm_bulk_f32(const mmssl_csr_t* a, const int32_t* buckets8
     cudaStream_t stream = (cudaStream_t)stream_;
     MMSSL_REQUIRE(a != nullptr && (buckets8 != nullptr || n_buckets == 0) && n_buckets >= 0, "missing bucket table (mmssl_spmm_bulk_plan)");
     MMSSL_REQUIRE(nrhs >= 1 && nrhs <= 2, "the staged-gather SpMM takes 1 or 2 right-hand sides");
+    if (d != 64 && d != 128 && d != 256) return fail_width("mmssl_spmm_bulk_f32 (64, 128 or 256 only)", d);
     BulkParams bp;
     mmssl_csr_t a2 = *a;            // the classic plan's item list is not used here: only the split table / counters of the bucket plan
     a2.n_items = 0;
@@ -467,6 +468,7 @@ extern "C" int mmssl_spmm_bulk_f32(const mmssl_csr_t* a, const int32_t* buckets8
     return tma ? launch_bulk<V, 2, true>(bp, stream, wpb, tpw) : launch_bulk<V, 2, false>(bp, stream, wpb, tpw);
     if (d == 64) { MMSSL_BULK_CASE(2) }
     if (d == 128) { MMSSL_BULK_CASE(4) }
-    MMSSL_BULK_CASE(8)
+    if (d == 256) { MMSSL_BULK_CASE(8) }
 #undef MMSSL_BULK_CASE
+    return fail_width(__func__, d);
 }

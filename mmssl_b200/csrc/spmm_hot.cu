@@ -249,8 +249,9 @@ int launch_spmm_hot(const SpmmParams& p, int d, int nrhs, const int32_t* colidx_
     }
     if (d == 64) { MMSSL_HOT_CASE(16, 1) }
     if (d == 128) { MMSSL_HOT_CASE(32, 1) }
-    MMSSL_HOT_CASE(32, 2)
+    if (d == 256) { MMSSL_HOT_CASE(32, 2) }
 #undef MMSSL_HOT_CASE
+    return fail_width("the hot-row SpMM (64, 128 or 256 only)", d);
 }
 
 }  // namespace mmssl
@@ -262,6 +263,7 @@ extern "C" int mmssl_spmm_hot_f32(const mmssl_csr_t* a, const int32_t* colidx_ho
                                   float* partials, int64_t partials_floats, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     MMSSL_REQUIRE(colidx_hot != nullptr && hot_ids != nullptr && n_hot >= 0, "missing hot-column plan");
+    if (d != 64 && d != 128 && d != 256) return fail_width("mmssl_spmm_hot_f32 (64, 128 or 256 only)", d);
     SpmmParams p;
     if (int rc = fill_spmm_params(p, a, d, nrhs, rhs, epilogue, alpha, s_mode, partials, partials_floats)) return rc;
     for (int r = 0; r < nrhs; ++r) MMSSL_REQUIRE(p.ldx[r] % 4 == 0, "TMA staging needs 16-byte aligned rows");

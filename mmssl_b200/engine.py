@@ -19,12 +19,13 @@ import os
 
 import torch
 
-from . import ops
+from . import _lib, ops
 from .graph import BipartiteGraph
 
 P_WV, P_BV, P_WT, P_BT = "image_trans.weight", "image_trans.bias", "text_trans.weight", "text_trans.bias"
 P_EU, P_EI, P_WCAT = "user_id_embedding.weight", "item_id_embedding.weight", "weight_dict.w_self_attention_cat"
 LIVE = (P_WV, P_BV, P_WT, P_BT, P_EU, P_EI, P_WCAT)
+SUPPORTED_WIDTHS = (32, 64, 96, 128, 192, 256)   # for messages; the library's mmssl_embed_width_supported decides
 
 
 class FeatureStore:
@@ -72,8 +73,8 @@ def _prio(name: str, default: int) -> int:
 class Engine:
     def __init__(self, embed_size: int, n_layers: int, head_num: int = 4, id_cat_rate: float = 0.36,
                  model_cat_rate: float = 0.55, proj_impl: str = "tc"):
-        if embed_size not in (64, 128, 256):
-            raise ValueError("mmssl_b200 kernels are built for embed_size 64, 128 or 256")
+        if not _lib.load().mmssl_embed_width_supported(int(embed_size)):
+            raise ValueError(f"embed_size {embed_size} is not supported: mmssl_b200 kernels are built for {SUPPORTED_WIDTHS}")
         self.d, self.K, self.H = embed_size, n_layers, head_num
         self.id_rate, self.cat_rate = id_cat_rate, model_cat_rate
         self.proj_impl = proj_impl
@@ -277,7 +278,8 @@ class Engine:
 
                 def fuse(ya, yb, e):
                     return ops.id_fuse2_fwd(ya, None if ya is yb else yb, 1.0 if ya is yb else 0.5, st.wsum, e, self.id_rate)
-            else:                   # d = 256: the d x d matrix does not fit shared memory -> GEMM path
+            else:                   # d = 32, 96, 192, 256: no fused kernel at these widths (the d x d matrix of 256 does not fit
+                                    # shared memory) -> GEMM path
                 st.wsum = ops.sgemm(self._tile(dev), P[P_WCAT], self._new(d, d, dev=dev))
 
                 def fuse(ya, yb, e):
