@@ -26,14 +26,18 @@ namespace mmssl {
 static constexpr int ctas_per_sm(int64_t n) { return n <= 64 ? 2 : 1; }
 static bool proj_width_ok(int64_t n) { return n == 32 || n == 64 || n == 96 || n == 128 || n == 192 || n == 256; }
 
-template <int N>
+// kDeep: the one-CTA-per-SM instance of the grouped kernel at N = 32 / 64, which spends the whole SM's shared memory on its
+// ring: 5 x 40 KB / 4 x 48 KB, so three to four k-blocks of F (32 KB each) are in flight per SM instead of one.
+template <int N, bool kDeep = false>
 struct GemmCfg {
     static constexpr int kTileBBytes = N * kBlockK * 2;
     static constexpr int kStageBytes = 2 * kTileABytes + 2 * kTileBBytes;   // 32 KB of A (hi + lo) + N * 256 B of B
-    static constexpr int kCtasPerSm = ctas_per_sm(N);
+    static constexpr int kCtasPerSm = kDeep ? 1 : ctas_per_sm(N);
     // 2 x 40 / 48 KB per CTA at N = 32 / 64; 3 x 56 / 64 KB at N = 96 / 128; 2 x 80 / 128 KB at N = 192 / 256
-    static constexpr int kStages = (N <= 64) ? 2 : (N <= 128 ? 3 : 2);
+    static constexpr int kStages = kDeep ? (N <= 32 ? 5 : 4) : (N <= 64) ? 2 : (N <= 128 ? 3 : 2);
     static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert(!kDeep || N <= 64, "the deep instance exists for N = 32 and 64 only");
+    static_assert(kSmemBytes <= 227 * 1024, "shared memory of one CTA");
 };
 constexpr int kGroupMax = 2;                                                // problems of one grouped launch (image, text)
 
@@ -168,10 +172,10 @@ __host__ __device__ __forceinline__ GroupUnit group_unit(const GroupClass* cls, 
     return w;
 }
 
-template <int N>
-__global__ void __launch_bounds__(kThreads, GemmCfg<N>::kCtasPerSm)
+template <int N, bool kDeep>
+__global__ void __launch_bounds__(kThreads, GemmCfg<N, kDeep>::kCtasPerSm)
 gemm_bf16x3_group_kernel(const __grid_constant__ GroupParams P) {
-    using Cfg = GemmCfg<N>;
+    using Cfg = GemmCfg<N, kDeep>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
@@ -360,15 +364,15 @@ static int group_check_shapes(int np, const int64_t* m, const int64_t* n, const 
     return 0;
 }
 
-template <int N>
+template <int N, bool kDeep = false>
 static int launch_group(const GroupParams& prm, int grid, cudaStream_t st) {
-    using Cfg = GemmCfg<N>;
+    using Cfg = GemmCfg<N, kDeep>;
     static bool attr_done = false;
     if (!attr_done) {
-        MMSSL_CUDA(cudaFuncSetAttribute(gemm_bf16x3_group_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+        MMSSL_CUDA(cudaFuncSetAttribute(gemm_bf16x3_group_kernel<N, kDeep>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
         attr_done = true;
     }
-    gemm_bf16x3_group_kernel<N><<<grid, kThreads, Cfg::kSmemBytes, st>>>(prm);
+    gemm_bf16x3_group_kernel<N, kDeep><<<grid, kThreads, Cfg::kSmemBytes, st>>>(prm);
     MMSSL_LAUNCH_OK();
     return 0;
 }
@@ -439,9 +443,11 @@ extern "C" int mmssl_gemm_bf16x3_group(int n_problems, const mmssl_gemm_problem_
     prm.n_classes = group_classes(n_problems, m, n, k, split, partial, prm.cls);
     prm.n_units = prm.cls[prm.n_classes - 1].u0 + prm.cls[prm.n_classes - 1].n_units;
     const int grid = group_grid(prm.n_units, (int)n[0], max_ctas);
+    // at most one CTA per SM (the engine's 132-CTA cap): the deep-ring instance, which fills the SM's shared memory alone
+    const bool deep = grid <= kNumSMs;
     switch (n[0]) {
-        case 32: return launch_group<32>(prm, grid, st);
-        case 64: return launch_group<64>(prm, grid, st);
+        case 32: return deep ? launch_group<32, true>(prm, grid, st) : launch_group<32>(prm, grid, st);
+        case 64: return deep ? launch_group<64, true>(prm, grid, st) : launch_group<64>(prm, grid, st);
         case 96: return launch_group<96>(prm, grid, st);
         case 128: return launch_group<128>(prm, grid, st);
         case 192: return launch_group<192>(prm, grid, st);

@@ -173,13 +173,16 @@ class Engine:
         return torch.empty(*shape, dtype=torch.float32, device=dev)
 
     # ------------------------------------------------------------------ projection
-    def _project(self, P, feats, masks, ys):
+    def _project(self, P, feats, masks, ys, join=None):
         """X = F W^T + b, then the dropout mask, for image and text (Models.py:173-174).  Tensor cores: both GEMMs in ONE
         grouped persistent launch (the feature streams of 118 + 30 MB at Baby share one balanced wave), then the two
-        split-K epilogues."""
+        split-K epilogues.  `join`: a stream whose work (the mask draws) the epilogues wait for; the GEMM does not."""
         d = self.d
         ws, bs = (P[P_WV], P[P_WT]), (P[P_BV], P[P_BT])
+        cur = torch.cuda.current_stream(ys[0].device)
         if self.proj_impl != "tc":
+            if join is not None and join is not cur:
+                cur.wait_stream(join)
             self._fork2(ys[0].device, lambda: self._project_simt(ws[0], bs[0], feats[0], masks[0], ys[0]),
                         lambda: self._project_simt(ws[1], bs[1], feats[1], masks[1], ys[1]))
             return
@@ -190,6 +193,8 @@ class Engine:
             w_hi, w_lo = ops.split_bf16(w)
             probs.append((fs.hi, fs.lo, w_hi, w_lo, fs.n_items, d, fs.dim, sk, part))
         ops.gemm_bf16x3_group(probs, self.proj_max_ctas)
+        if join is not None and join is not cur:
+            cur.wait_stream(join)
         for b, fs, sk, part, mask, y in zip(bs, feats, splits, parts, masks, ys):
             ops.proj_epilogue(part, sk, fs.n_items, d, b, mask, y)
 
@@ -230,7 +235,8 @@ class Engine:
     def forward(self, P: Dict[str, torch.Tensor], feats: Tuple[FeatureStore, FeatureStore],
                 graphs: Sequence[BipartiteGraph], masks, want_sumsq: bool = True, side_pre=None):
         """masks: None, a pair of [I, d] keep-masks (0 or 1/(1-p)), or a callable returning one -- the
-        callable and `side_pre` run at the head of the modality branch, i.e. off the critical path."""
+        callable and `side_pre` run on a branch forked at the head of the modality branch, i.e. off the critical path: the
+        projection GEMM starts at once, and only its epilogues (which apply the masks) wait for that branch."""
         g_ui, g_iu, g_vui, g_viu, g_tui, g_tiu = graphs
         U, I = g_ui.shape
         d, K = self.d, self.K
@@ -246,11 +252,18 @@ class Engine:
         resolved = [masks]
 
         def modal_branch():
-            if side_pre is not None:
-                side_pre()
-            m = masks() if callable(masks) else masks
+            cur = torch.cuda.current_stream(dev)
+            pre = cur
+            if self.two_streams and (side_pre is not None or callable(masks)):
+                pre = self._named_stream(dev, "pre")
+                pre.wait_stream(cur)
+            with torch.cuda.stream(pre):
+                if side_pre is not None:
+                    side_pre()
+                m = masks() if callable(masks) else masks
             resolved[0] = m
-            self._project(P, feats, m if m else (None, None), (xv, xt))                 # Models.py:173-174
+            # the modality branch joins the main stream before the loss kernels, so `pre` (seed memset, sampler) is joined too
+            self._project(P, feats, m if m else (None, None), (xv, xt), join=pre)       # Models.py:173-174
             self._spmm(g_ui, "fwd", [xv, xt], "i", [uv, ut])                        # :177,182
             self._spmm(g_iu, "fwd", [uv, ut], "u", [iv, it])                        # :178,183
 
