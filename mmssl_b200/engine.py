@@ -12,10 +12,9 @@ scheduled on three streams (see ``Engine.two_streams``).
 """
 from __future__ import annotations
 
+import contextlib
 from dataclasses import dataclass
 from typing import Dict, Optional, Sequence, Tuple
-
-import os
 
 import torch
 
@@ -64,10 +63,50 @@ class FwdState:
     sumsq_i: Optional[torch.Tensor] = None
 
 
+# The branches of the step and the priority of each one's stream (0 = lowest .. -5): the item-side twin of the critical id / GCN
+# chain ("pair") and the two side products of the tensor-core InfoNCE backward run ahead of the projection branch ("side").
+PRIORITY = {"side": 0, "pair": -1, "fork2": 0, "fork3": 0, "pre": 0, "loss": 0, "nce2": -1, "nce3": -1}
+_streams: Dict[Tuple, torch.cuda.Stream] = {}
 
-def _prio(name: str, default: int) -> int:
-    """Stream priority of one branch of the step (0 = lowest .. -5); MMSSL_PRIO_<NAME> overrides the measured default."""
-    return int(os.environ.get("MMSSL_PRIO_" + name, default))
+
+@contextlib.contextmanager
+def branch(dev, name: str, on: bool = True):
+    """Fork branch `name` of the step: the body is issued on that branch's stream (one per device and name), after the work
+    issued so far on the current stream.  Yields the stream for `join`, which the caller places where the branch's results are
+    needed.  With `on` False the body runs on the current stream and None is yielded."""
+    if not on:
+        yield None
+        return
+    key = (dev.type, dev.index, name)
+    st = _streams.get(key)
+    if st is None:
+        st = _streams[key] = torch.cuda.Stream(device=dev, priority=PRIORITY[name])
+    st.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(st):
+        yield st
+
+
+def join(dev, *branches) -> None:
+    """The current stream waits for the work issued so far on `branches` (None stands for a branch that ran inline)."""
+    cur = torch.cuda.current_stream(dev)
+    for st in branches:
+        if st is not None:
+            cur.wait_stream(st)
+
+
+def capture_graph(warmup, body):
+    """Runs `warmup` on a stream forked from the current one (so that every lazily created buffer and stream exists), waits for
+    the device, then captures `body` into a CUDA graph.  Returns (graph, what `body` returned)."""
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        warmup()
+    torch.cuda.current_stream().wait_stream(s)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        out = body()
+    return g, out
 
 
 class Engine:
@@ -80,14 +119,13 @@ class Engine:
         self.proj_impl = proj_impl
         # Grid of the grouped projection GEMM: one CTA per SM (132 on the H100 SXM) rather than the full two-per-SM wave.  The
         # persistent CTAs would otherwise hold every slot while the id / GCN branch runs beside them; measured on an H100 at
-        # 700 W, 132 CTAs gave the shorter Baby and Sports steps (DESIGN section 6).  MMSSL_PROJ_MAX_CTAS overrides it (0 = full wave).
-        self.proj_max_ctas = int(os.environ.get("MMSSL_PROJ_MAX_CTAS", 132))
+        # 700 W, 132 CTAs gave the shorter Baby and Sports steps (DESIGN section 6).
+        self.proj_max_ctas = 132
         self._tile_id: Dict[Tuple, torch.Tensor] = {}
         # The modality branch (projection -> A_ui [Xv|Xt] -> A_iu [Uv|Ut]) and the id/GCN branch are
         # independent until the final combine (and again after combine-backward), so they run on two
         # streams; inside a CUDA graph they become parallel branches.  Set to False to serialise.
         self.two_streams = True
-        self._side: Dict[Tuple, torch.cuda.Stream] = {}
         # Row-sharded scheme (SURVEY 8e, rowshard_step.py): every table is a row block, the graphs are row blocks with
         # global column ids, and each SpMM needs its dense operand from all ranks.  ``exchange(list_of_local, space)``
         # ('u' = user rows, 'i' = item rows) returns the gathered operands; None = single GPU, operands pass through.
@@ -106,58 +144,20 @@ class Engine:
             return self.sharded_spmm(g, which, xs, space, ys, **kw)
         return ops.spmm(getattr(g, which), self._full(xs, space), ys, **kw)
 
-    def _pair(self, dev, fn_a, fn_b):
-        """Run two independent kernel groups concurrently (user side on the current stream, item side
-        on the 'pair' stream) and join.  Returns (fn_a(), fn_b())."""
+    def branch(self, dev, name: str, on: bool = True):
+        """`branch` of this engine's schedule: inline when `two_streams` is off."""
+        return branch(dev, name, on and self.two_streams)
+
+    def _fork(self, dev, name: str, fn_a, fn_b):
+        """Two independent kernel groups: fn_a on the current stream, fn_b beside it on branch `name`, joined at once (a, then b,
+        on one stream when `two_streams` is off).  Returns (fn_a(), fn_b())."""
         if not self.two_streams:
             return fn_a(), fn_b()
-        key = (dev.type, dev.index, "pair")
-        st = self._side.get(key)
-        if st is None:
-            st = torch.cuda.Stream(device=dev, priority=_prio("PAIR", -1))      # twin of the critical id / GCN chain: ahead of the projection branch
-            self._side[key] = st
-        main = torch.cuda.current_stream(dev)
-        st.wait_stream(main)
-        with torch.cuda.stream(st):
+        with branch(dev, name) as st:
             rb = fn_b()
         ra = fn_a()
-        main.wait_stream(st)
+        join(dev, st)
         return ra, rb
-
-    def _fork2(self, dev, fn_a, fn_b, name: str = "fork2"):
-        """fn_a on the current stream, fn_b on a third stream (forked from / joined into the current one); serial when
-        `two_streams` is off.  Used for the image | text halves of the projection, which are independent."""
-        if not self.two_streams:
-            fn_a(); fn_b()
-            return
-        key = (dev.type, dev.index, name)
-        st = self._side.get(key)
-        if st is None:
-            st = torch.cuda.Stream(device=dev, priority=_prio("FORK", 0))
-            self._side[key] = st
-        cur = torch.cuda.current_stream(dev)
-        st.wait_stream(cur)
-        with torch.cuda.stream(st):
-            fn_b()
-        fn_a()
-        cur.wait_stream(st)
-
-    def _named_stream(self, dev, name: str) -> torch.cuda.Stream:
-        """One more branch of the step (the caller forks it from and joins it into the main stream)."""
-        key = (dev.type, dev.index, name)
-        st = self._side.get(key)
-        if st is None:
-            st = torch.cuda.Stream(device=dev, priority=_prio(name.upper(), 0))
-            self._side[key] = st
-        return st
-
-    def _side_stream(self, dev) -> torch.cuda.Stream:
-        key = (dev.type, dev.index)
-        st = self._side.get(key)
-        if st is None:
-            st = torch.cuda.Stream(device=dev, priority=_prio("SIDE", 0))
-            self._side[key] = st
-        return st
 
     # ------------------------------------------------------------------ helpers
     def _tile(self, dev) -> torch.Tensor:
@@ -173,28 +173,26 @@ class Engine:
         return torch.empty(*shape, dtype=torch.float32, device=dev)
 
     # ------------------------------------------------------------------ projection
-    def _project(self, P, feats, masks, ys, join=None):
+    def _project(self, P, feats, masks, ys, wait_for=None):
         """X = F W^T + b, then the dropout mask, for image and text (Models.py:173-174).  Tensor cores: both GEMMs in ONE
         grouped persistent launch (the feature streams of 118 + 30 MB at Baby share one balanced wave), then the two
-        split-K epilogues.  `join`: a stream whose work (the mask draws) the epilogues wait for; the GEMM does not."""
+        split-K epilogues.  `wait_for`: a branch whose work (the mask draws) the epilogues wait for; the GEMM does not."""
         d = self.d
+        dev = ys[0].device
         ws, bs = (P[P_WV], P[P_WT]), (P[P_BV], P[P_BT])
-        cur = torch.cuda.current_stream(ys[0].device)
         if self.proj_impl != "tc":
-            if join is not None and join is not cur:
-                cur.wait_stream(join)
-            self._fork2(ys[0].device, lambda: self._project_simt(ws[0], bs[0], feats[0], masks[0], ys[0]),
-                        lambda: self._project_simt(ws[1], bs[1], feats[1], masks[1], ys[1]))
+            join(dev, wait_for)
+            self._fork(dev, "fork2", lambda: self._project_simt(ws[0], bs[0], feats[0], masks[0], ys[0]),
+                       lambda: self._project_simt(ws[1], bs[1], feats[1], masks[1], ys[1]))
             return
         splits, floats = ops.gemm_bf16x3_group_plan([(fs.n_items, d, fs.dim) for fs in feats], self.proj_max_ctas)
-        parts = self._new(sum(floats), dev=ys[0].device).split(floats)
+        parts = self._new(sum(floats), dev=dev).split(floats)
         probs = []
         for w, fs, sk, part in zip(ws, feats, splits, parts):
             w_hi, w_lo = ops.split_bf16(w)
             probs.append((fs.hi, fs.lo, w_hi, w_lo, fs.n_items, d, fs.dim, sk, part))
         ops.gemm_bf16x3_group(probs, self.proj_max_ctas)
-        if join is not None and join is not cur:
-            cur.wait_stream(join)
+        join(dev, wait_for)
         for b, fs, sk, part, mask, y in zip(bs, feats, splits, parts, masks, ys):
             ops.proj_epilogue(part, sk, fs.n_items, d, b, mask, y)
 
@@ -211,8 +209,8 @@ class Engine:
         the same pass), both weight-gradient GEMMs in ONE grouped persistent launch, then the two epilogues."""
         d = self.d
         if self.proj_impl != "tc":
-            self._fork2(gxs[0].device, lambda: self._project_bwd_simt(gxs[0], masks[0], feats[0], dws[0], dbs[0]),
-                        lambda: self._project_bwd_simt(gxs[1], masks[1], feats[1], dws[1], dbs[1]))
+            self._fork(gxs[0].device, "fork2", lambda: self._project_bwd_simt(gxs[0], masks[0], feats[0], dws[0], dbs[0]),
+                       lambda: self._project_bwd_simt(gxs[1], masks[1], feats[1], dws[1], dbs[1]))
             return
         splits, floats = ops.gemm_bf16x3_group_plan([(fs.dim, d, fs.n_items) for fs in feats], self.proj_max_ctas)
         parts = self._new(sum(floats), dev=gxs[0].device).split(floats)
@@ -246,33 +244,16 @@ class Engine:
         xv, xt = X2[:, :d], X2[:, d:]
         uv, ut = U2[:, :d], U2[:, d:]
         iv, it = I2[:, :d], I2[:, d:]
-        main = torch.cuda.current_stream(dev)
-        side = self._side_stream(dev) if self.two_streams else main
 
-        resolved = [masks]
-
-        def modal_branch():
-            cur = torch.cuda.current_stream(dev)
-            pre = cur
-            if self.two_streams and (side_pre is not None or callable(masks)):
-                pre = self._named_stream(dev, "pre")
-                pre.wait_stream(cur)
-            with torch.cuda.stream(pre):
+        with self.branch(dev, "side") as side:                                      # the modality branch
+            with self.branch(dev, "pre", on=side_pre is not None or callable(masks)) as pre:
                 if side_pre is not None:
                     side_pre()
                 m = masks() if callable(masks) else masks
-            resolved[0] = m
             # the modality branch joins the main stream before the loss kernels, so `pre` (seed memset, sampler) is joined too
-            self._project(P, feats, m if m else (None, None), (xv, xt), join=pre)       # Models.py:173-174
+            self._project(P, feats, m if m else (None, None), (xv, xt), wait_for=pre)   # Models.py:173-174
             self._spmm(g_ui, "fwd", [xv, xt], "i", [uv, ut])                        # :177,182
             self._spmm(g_iu, "fwd", [uv, ut], "u", [iv, it])                        # :178,183
-
-        if side is not main:
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                modal_branch()
-        else:
-            modal_branch()
 
         def id_prop(ga, gb, e, rows, space):                                           # :179-180,185-186
             def one(g):
@@ -282,8 +263,9 @@ class Engine:
             ya = one(ga)
             return (ya, ya) if ga is gb else (ya, one(gb))
 
-        (uvid, utid), (ivid, itid) = self._pair(dev, lambda: id_prop(g_vui, g_tui, e_i, U, "i"), lambda: id_prop(g_viu, g_tiu, e_u, I, "u"))
-        st = FwdState(tuple(graphs), resolved[0], X2, U2, I2, (uvid, utid, ivid, itid),
+        (uvid, utid), (ivid, itid) = self._fork(dev, "pair", lambda: id_prop(g_vui, g_tui, e_i, U, "i"),
+                                                lambda: id_prop(g_viu, g_tiu, e_u, I, "u"))
+        st = FwdState(tuple(graphs), m, X2, U2, I2, (uvid, utid, ivid, itid),
                       fused=any(g.nnz > 0 for g in (g_vui, g_viu, g_tui, g_tiu)))
         if st.fused:                                                                   # :188-197 (closed form)
             if d in (64, 128):      # fused row x matrix kernels, Wsum in shared memory
@@ -305,7 +287,8 @@ class Engine:
                     out = self._new(e.shape[0], d, dev=dev)
                     return ops.id_fuse_fwd(z, e, self.id_rate, out)
 
-            (u0, st.zn_u, st.nrm_u), (i0, st.zn_i, st.nrm_i) = self._pair(dev, lambda: fuse(uvid, utid, e_u), lambda: fuse(ivid, itid, e_i))
+            (u0, st.zn_u, st.nrm_u), (i0, st.zn_i, st.nrm_i) = self._fork(dev, "pair", lambda: fuse(uvid, utid, e_u),
+                                                                          lambda: fuse(ivid, itid, e_i))
         else:
             u0, i0 = e_u, e_i
         # GCN layers: u_{k+1} = A_ui i_k ; i_{k+1} = A_iu u_{k+1}; softmax on the last one (:201-211);
@@ -325,10 +308,9 @@ class Engine:
                 st.u_last, st.i_last = u_n, i_n
             cur_i = i_n
         inv = 1.0 / (K + 1)
-        if side is not main:
-            main.wait_stream(side)      # join: the combine needs Uv|Ut and Iv|It
-        (u_f, st.sumsq_u), (i_f, st.sumsq_i) = self._pair(
-            dev, lambda: ops.combine_fwd(s_u, uv, ut, inv, self.cat_rate, self._new(U, d, dev=dev), want_sumsq),      # :213,217
+        join(dev, side)                 # the combine needs Uv|Ut and Iv|It
+        (u_f, st.sumsq_u), (i_f, st.sumsq_i) = self._fork(
+            dev, "pair", lambda: ops.combine_fwd(s_u, uv, ut, inv, self.cat_rate, self._new(U, d, dev=dev), want_sumsq),      # :213,217
             lambda: ops.combine_fwd(s_i, iv, it, inv, self.cat_rate, self._new(I, d, dev=dev), want_sumsq))          # :214,218
         outs = (u_f, i_f, iv, it, uv, ut, uvid, utid, ivid, itid)
         return outs, st
@@ -373,13 +355,11 @@ class Engine:
         iv, it = st.I2[:, :d], st.I2[:, d:]
         # ---- combine backward (Models.py:213-218): through the two normalisations (+ feat_reg)
         gU2, gI2 = self._new(U, 2 * d, dev=dev), self._new(I, 2 * d, dev=dev)
-        self._pair(dev, lambda: ops.combine_bwd(g_uf, uv, ut, g_uv, g_ut, self.cat_rate, feat_reg_coef, gU2[:, :d], gU2[:, d:]),
+        self._fork(dev, "pair", lambda: ops.combine_bwd(g_uf, uv, ut, g_uv, g_ut, self.cat_rate, feat_reg_coef, gU2[:, :d], gU2[:, d:]),
                    lambda: ops.combine_bwd(g_if, iv, it, g_iv, g_it, self.cat_rate, feat_reg_coef, gI2[:, :d], gI2[:, d:]))
-        main = torch.cuda.current_stream(dev)
-        side = self._side_stream(dev) if self.two_streams else main
         w_slots = (slot(P_WV, P[P_WV]), slot(P_BV, P[P_BV]), slot(P_WT, P[P_WT]), slot(P_BT, P[P_BT]))
 
-        def modal_backward():
+        with self.branch(dev, "side") as side:
             # modality propagation backward (Models.py:177-178,182-183), image|text batched, then the
             # projection backward (dropout mask folded into the operand split)
             self._spmm(g_iu, "bwd", [gI2[:, :d], gI2[:, d:]], "i", [gU2[:, :d], gU2[:, d:]], cs=[gU2[:, :d], gU2[:, d:]], alpha=1.0)
@@ -388,14 +368,6 @@ class Engine:
             m = st.masks
             self._project_bwd((gX2[:, :d], gX2[:, d:]), m if m else (None, None), feats, (w_slots[0], w_slots[2]),
                               (w_slots[1], w_slots[3]))
-            return gX2
-
-        if side is not main:
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                keep = modal_backward()
-        else:
-            keep = modal_backward()
         # ---- GCN backward.  every u_k, i_k receives inv * g_uf / inv * g_if from the layer mean.
         # d loss / d u_0 = inv * g_uf (u_0 only feeds the layer mean): needed only after the chain -> issued first, on the pair stream
         g_eu = slot(P_EU, P[P_EU])
@@ -433,14 +405,15 @@ class Engine:
                 ops.axpby(g_uf, inv, 0.0, g_eu)
                 return fuse_bwd2(g_eu, st.zn_u, st.nrm_u, uvid, utid, g_uvid, g_utid)
 
-            _, (gt_uvid, gt_utid, part_u) = self._pair(dev, chain, user_side)
+            _, (gt_uvid, gt_utid, part_u) = self._fork(dev, "pair", chain, user_side)
             gt_ivid, gt_itid, part_i = fuse_bwd2(g_ei, st.zn_i, st.nrm_i, ivid, itid, g_ivid, g_itid)
             dwcat_args = (part_u, part_i)
         else:
-            self._pair(dev, chain, lambda: ops.axpby(g_uf, inv, 0.0, g_eu))
-        if fused2:
-            pass
-        elif st.fused:
+            self._fork(dev, "pair", chain, lambda: ops.axpby(g_uf, inv, 0.0, g_eu))
+        if not st.fused:
+            g_wcat.zero_()
+            gt_uvid, gt_utid, gt_ivid, gt_itid = g_uvid, g_utid, g_ivid, g_itid
+        elif not fused2:
             d_wsum = torch.zeros(d, d, dtype=torch.float32, device=dev)
 
             def fuse_bwd(g0, zn, nrm, ya, yb, g_ya, g_yb, rows):
@@ -460,7 +433,7 @@ class Engine:
                 ops.sgemm(dz, st.wsum, ta, trans_b=True, alpha=0.5)
                 tb = ta
                 if g_ya is not None or g_yb is not None:
-                    tb = ta.clone() if g_yb is not None or g_ya is not None else ta
+                    tb = ta.clone()
                     if g_ya is not None:
                         ops.axpby(g_ya, 1.0, 1.0, ta)
                     if g_yb is not None:
@@ -470,9 +443,6 @@ class Engine:
             gt_uvid, gt_utid = fuse_bwd(g_eu, st.zn_u, st.nrm_u, uvid, utid, g_uvid, g_utid, U)
             gt_ivid, gt_itid = fuse_bwd(g_ei, st.zn_i, st.nrm_i, ivid, itid, g_ivid, g_itid, I)
             ops.sgemm(self._tile(dev), d_wsum, g_wcat, trans_a=True)            # dWcat[h] = dWsum for every head
-        else:
-            g_wcat.zero_()
-            gt_uvid, gt_utid, gt_ivid, gt_itid = g_uvid, g_utid, g_ivid, g_itid
 
         def id_prop_bwd(ga, gb, gya, gyb, g_e, same_out, space):
             # E-gradient += A^T g  for each modality graph (same_out: both modalities share graph and output)
@@ -493,14 +463,13 @@ class Engine:
         # Uvid = A_vui E_i, Utid = A_tui E_i -> gradient flows to E_i; Ivid/Itid -> E_u.  The head reduction of dWcat feeds
         # nothing else of the step: it runs beside the two propagations on a third stream.
         def props():
-            self._pair(dev, lambda: id_prop_bwd(g_vui, g_tui, gt_uvid, gt_utid, g_ei, st.fused and uvid is utid, "u"),
+            self._fork(dev, "pair", lambda: id_prop_bwd(g_vui, g_tui, gt_uvid, gt_utid, g_ei, st.fused and uvid is utid, "u"),
                        lambda: id_prop_bwd(g_viu, g_tiu, gt_ivid, gt_itid, g_eu, st.fused and ivid is itid, "i"))
 
         def head_reduce():
             if dwcat_args is not None:
                 ops.dwcat_reduce(dwcat_args[0], dwcat_args[1], d, self.H, g_wcat)
 
-        self._fork2(dev, props, head_reduce, name="fork3")
-        if side is not main:
-            main.wait_stream(side)
+        self._fork(dev, "fork3", props, head_reduce)
+        join(dev, side)
         return res

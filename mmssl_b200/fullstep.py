@@ -36,7 +36,7 @@ import torch.nn.functional as F
 
 from . import _lib, gan
 from ._lib import ptr, stream
-from .engine import LIVE, FeatureStore
+from .engine import LIVE, FeatureStore, capture_graph
 from .graph import BipartiteGraph
 from .hotstep import HotStep, HotStepConfig
 
@@ -255,16 +255,15 @@ class FullStep:
         if not self.steady():
             raise RuntimeError("capture() needs the steady state: run the first iterations of the epoch eagerly")
         self._static = self._draws(None, None, None, None, None)
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):                           # warm-up: every lazily created buffer exists before the capture
+
+        def warm():
             self._body(*self._static)
             self.idx += 1
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        step_before = self.D.step
-        with torch.cuda.graph(g):
-            self._static_out = self._body(*self._static)
-        self.D.step = step_before                            # the capture pass does not execute
-        self._graph = g
+
+        def body():
+            step_before = self.D.step
+            out = self._body(*self._static)
+            self.D.step = step_before                        # the capture pass does not execute
+            return out
+
+        self._graph, self._static_out = capture_graph(warm, body)

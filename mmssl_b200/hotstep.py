@@ -18,7 +18,7 @@ import torch
 import torch.nn.functional as F
 
 from . import ops
-from .engine import LIVE, P_EI, P_EU, Engine, FeatureStore
+from .engine import LIVE, P_EI, P_EU, Engine, FeatureStore, capture_graph, join
 from .graph import BipartiteGraph
 
 
@@ -114,11 +114,7 @@ class HotStep:
         reg_coef = cfg.emb_decay / cfg.batch_size
         # BPR: value partials + gradient rows scattered straight into the dense table gradients
         dev = u_f.device
-        main = torch.cuda.current_stream(dev)
-        side = self.engine._side_stream(dev) if self.engine.two_streams else main
-        if side is not main:        # BPR runs next to InfoNCE (both only add into the seed buffers, atomically)
-            side.wait_stream(main)
-        with torch.cuda.stream(side):
+        with self.engine.branch(dev, "side") as side:     # BPR runs next to InfoNCE (both only add into the seed buffers, atomically)
             bpr_part, n_bpr = ops.bpr(u_f, i_f, i_f, users, pos, neg, mode=3, reg_coef=reg_coef,
                                       g_u=self.g_uf, g_p=self.g_if, g_n=self.g_if)
         # InfoNCE(Uvid[users], u_f[users]) + InfoNCE(Utid[users], u_f[users])   (main.py:411-412)
@@ -128,15 +124,11 @@ class HotStep:
             parts.append(ops.infonce_forward(z1, u_f, users, inv_tau, w, g_loss=self.cl_seed))
             if st.fused:    # with empty modality graphs z1 == 0: the loss is a constant, all gradients vanish
                 ops.infonce_backward(users, inv_tau, w, gz1, self.g_uf)
-        if side is not main:
-            main.wait_stream(side)
+        join(dev, side)
         nce1 = parts[0]
         nce2 = parts[0] if self.alias_id else parts[1]
         # the five loss VALUES feed nothing of the backward: assembled on a stream of their own, joined at the end of the step
-        loss_st = self.engine._named_stream(dev, "loss") if self.engine.two_streams else main
-        if loss_st is not main:
-            loss_st.wait_stream(main)
-        with torch.cuda.stream(loss_st):
+        with self.engine.branch(dev, "loss") as loss_st:
             ops.loss_assemble(bpr_part, n_bpr, self.batch, reg_coef, st.sumsq_u, st.sumsq_i, 0.5 * cfg.feat_reg_decay / self.I,
                               nce1, nce2, self.batch, cfg.cl_rate, self.out5)
         extra = self.post_forward(outs, st) if self.post_forward is not None else (None, None, None, None)
@@ -150,25 +142,17 @@ class HotStep:
             keys = list(LIVE)
             ops.adamw([self.P[k] for k in keys], [self.grads[k] for k in keys], [self.m[k] for k in keys],
                       [self.v[k] for k in keys], self.step_dev, cfg.lr, cfg.beta1, cfg.beta2, cfg.eps, cfg.weight_decay)
-        if loss_st is not main:
-            main.wait_stream(loss_st)
+        join(dev, loss_st)
         return self.out5
 
     # ------------------------------------------------------------------ CUDA graph
     def capture(self, warmup: int = 2) -> None:
         """Capture ``run`` into a CUDA graph (static buffers; update ``self.idx`` between replays).
         Warm-up steps run on a side stream first and DO advance the optimiser state."""
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
+        def warm():
             for _ in range(warmup):
                 self.run()
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self.run()
-        self._graph = g
+        self._graph, _ = capture_graph(warm, self.run)
 
     def replay(self) -> torch.Tensor:
         if self._graph is None:

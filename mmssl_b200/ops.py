@@ -247,16 +247,6 @@ def bpr(uf, pf, nf, users, pos, neg, *, mode: int, reg_coef: float, g_mf=None, g
 
 
 NCE_STREAMS = True      # tensor-core backward: its three products on three streams
-_nce_streams = {}
-
-
-def _nce_side_streams(dev):
-    key = (dev.type, dev.index)
-    if key not in _nce_streams:
-        _nce_streams[key] = (torch.cuda.Stream(device=dev, priority=-1), torch.cuda.Stream(device=dev, priority=-1))
-    return _nce_streams[key]
-
-
 NCE_IMPL = "auto"       # "auto": tensor cores where mmssl_infonce_tc_supported (n <= 2048, d in {64, 128}); "simt": CUDA cores
 
 
@@ -292,11 +282,8 @@ def infonce_forward(z1, z2, idx, inv_tau: float, work: InfoNCEWork, g_loss=None)
         return work.loss_part[:work.n_loss_blocks]
     _lib.check(lib.mmssl_infonce_prepare(ptr(z1), _ld(z1), ptr(z2), _ld(z2), ptr(idx), n, d, ptr(work.a), ptr(work.b),
                                          ptr(work.na), ptr(work.nb), ptr(work.ga), ptr(work.gb), stream()))
-    if False:
-        pass
-    else:
-        _lib.check(lib.mmssl_infonce_stats(ptr(work.a), ptr(work.b), n, d, float(inv_tau), ptr(work.stats), ptr(work.coef),
-                                           ptr(g_loss), ptr(work.loss_part), stream()))
+    _lib.check(lib.mmssl_infonce_stats(ptr(work.a), ptr(work.b), n, d, float(inv_tau), ptr(work.stats), ptr(work.coef),
+                                       ptr(g_loss), ptr(work.loss_part), stream()))
     return work.loss_part[:work.n_loss_blocks]
 
 
@@ -308,18 +295,17 @@ def infonce_backward(idx, inv_tau: float, work: InfoNCEWork, g_z1, g_z2):
         def phase(p):
             _lib.check(lib.mmssl_infonce_grad_tc(ptr(work.a), ptr(work.b), n, d, float(inv_tau), ptr(work.coef), ptr(work.stats),
                                                  ptr(work.ga), ptr(work.gb), ptr(work.ws), work.ws.numel(), p, stream()))
-        if work.a.is_cuda and NCE_STREAMS and torch.cuda.is_available():
-            # the three products are independent: two of them on side streams (forked / joined by events, graph-capturable)
+        if NCE_STREAMS:
+            # the three products are independent: two of them on branches of their own (graph-capturable)
+            from .engine import branch, join        # engine imports this module
+            dev = work.a.device
             phase(0)
-            cur = torch.cuda.current_stream(work.a.device)
-            sides = _nce_side_streams(work.a.device)
-            for s_, p in zip(sides, (2, 3)):
-                s_.wait_stream(cur)
-                with torch.cuda.stream(s_):
-                    phase(p)
+            with branch(dev, "nce2") as s2:
+                phase(2)
+            with branch(dev, "nce3") as s3:
+                phase(3)
             phase(1)
-            for s_ in sides:
-                cur.wait_stream(s_)
+            join(dev, s2, s3)
             phase(4)
         else:
             phase(-1)

@@ -28,7 +28,7 @@ import torch.distributed as dist
 
 from . import _lib, ops
 from ._lib import ptr, stream
-from .engine import LIVE, P_EI, P_EU, Engine, FeatureStore
+from .engine import LIVE, P_EI, P_EU, Engine, FeatureStore, capture_graph
 from .graph import SparseOperand
 from .hotstep import HotStepConfig
 from .parallel import RowPartition, all_gather_rows, shard_rows_scipy
@@ -292,6 +292,7 @@ class RowShardedHotStep:
         self.step_dev = torch.zeros(1, dtype=torch.int32, device=dev)
         self.masks: Optional[tuple] = None                  # injected [I_block, d] keep-masks of the rank's item rows
         self.training = True
+        self._graph: Optional[torch.cuda.CUDAGraph] = None
         # the small replicated gradients travel in one flat buffer
         n = sum((self.grads[k].numel() + 3) // 4 * 4 for k in REPLICATED) + 4      # + one slot for the local feat_reg term
         self._feat_slot = n - 4
@@ -449,8 +450,7 @@ class RowShardedHotStep:
                       self.step_dev, cfg.lr, cfg.beta1, cfg.beta2, cfg.eps, cfg.weight_decay)
         return self.out5
 
-
-def _capture_methods():
+    # -------------------------------------------------------------- CUDA graph
     def capture(self, warmup: int = 2) -> None:
         """Capture ``run`` into a CUDA graph (static buffers; update the indices with ``set_indices`` between replays).  Only with the
         multicast exchange or a single rank: every exchange is then a kernel plus a device-side signal-pad barrier, which a graph
@@ -459,27 +459,17 @@ def _capture_methods():
             raise RuntimeError("capture() needs exchange='multicast' (NCCL collectives are not captured)")
         if self.pu.world > 1 and self.ar_rows is None:
             raise RuntimeError("capture() needs the multicast all-reduce (no NVSwitch multicast address on this system)")
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
+
+        def warm():
             for _ in range(warmup):
                 self.run()
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self.run()
-        self._graph = g
+        self._graph, _ = capture_graph(warm, self.run)
 
     def replay(self) -> torch.Tensor:
-        if getattr(self, "_graph", None) is None:
+        if self._graph is None:
             raise RuntimeError("call capture() first")
         self._graph.replay()
         return self.out5
-    return capture, replay
-
-
-RowShardedHotStep.capture, RowShardedHotStep.replay = _capture_methods()
 
 
 def shard_problem(P_full: Dict[str, torch.Tensor], feats_full: Sequence[torch.Tensor], ui_norm, iu_norm, rank: int, world: int, device):
