@@ -111,6 +111,8 @@ class FullStep:
             self.K.register_weights([self.D.t["net.0.weight"], self.D.t["net.4.weight"]])
         self.idx = 0                                    # iteration inside the epoch (main.py:333)
         self.pairs: Dict[str, List[Tuple[torch.Tensor, torch.Tensor]]] = {"image": [], "text": []}
+        # (x, y) pair lists the current modality graphs were built from; None: still the training graphs of step 0
+        self.graph_pairs: Dict[str, Optional[Tuple[torch.Tensor, torch.Tensor]]] = {"image": None, "text": None}
         self.k = int(self.I * cfg.m_topk_rate)
         dev = self.hs.P[LIVE[0]].device
         f = dict(dtype=torch.float32, device=dev)
@@ -173,6 +175,7 @@ class FullStep:
             if not self.pairs["image"] and not self.pairs["text"] and all(g.nnz == 0 for g in self.hs.graphs[2:]):
                 return                                   # empty lists onto already empty graphs: nothing changes (steady state at T = 1)
             new = list(self.hs.graphs)
+            self._new_pairs = {}
             for j, key in ((2, "image"), (4, "text")):
                 xs = [p[0] for p in self.pairs[key]]
                 ys = [p[1] for p in self.pairs[key]]
@@ -180,6 +183,7 @@ class FullStep:
                 x = torch.cat(xs) if xs else e
                 y = torch.cat(ys) if ys else e
                 new[j], new[j + 1] = graphs_from_pairs(x, y, self.U, self.I)
+                self._new_pairs[key] = (x, y)
             self.pairs = {"image": [], "text": []}
             self._new_graphs = tuple(new)
         elif self.k > 0:
@@ -225,8 +229,48 @@ class FullStep:
         out = self._body(*draws)
         if self._new_graphs is not None:
             self.hs.graphs = self._new_graphs
+            self.graph_pairs = self._new_pairs
         self.idx += 1
         return out
+
+    # -------------------------------------------------------------- checkpoint (checkpoint.py)
+    def state_dict(self) -> dict:
+        """HotStep state + the Discriminator and its Adam state + the epoch bookkeeping: iteration in the epoch, collected
+        pairs, and the pair lists the modality graphs were built from (the graphs are rebuilt from them on load)."""
+        st = self.hs.state_dict()
+        st.update(kind="fullstep", D=self.D.state_dict(), D_optim=self.D.optim_state_dict(),
+                  fullstep=dict(idx=int(self.idx), pairs={k: [tuple(p) for p in v] for k, v in self.pairs.items()},
+                                graph_pairs=dict(self.graph_pairs)))
+        return st
+
+    def load_state_dict(self, state: dict) -> None:
+        """In place, like HotStep.load_state_dict.  A captured iteration survives the load when the modality graphs stay the
+        ones it was recorded with; otherwise it is dropped (Trainer re-captures once ``steady()`` holds again)."""
+        from . import checkpoint
+        checkpoint.check_format(state, ("fullstep", "trainer"))
+        checkpoint.check_meta(state["meta"], self.hs.meta())
+        fs = state["fullstep"]
+        self.hs.load_state_dict(state)
+        self.D.load_state_dict(state["D"], state["D_optim"])
+        dev = self.gsim.device
+        on = lambda p: (p[0].to(dev), p[1].to(dev))
+        self.idx = int(fs["idx"])
+        self.pairs = {k: [on(p) for p in fs["pairs"][k]] for k in ("image", "text")}
+        want = {k: (None if fs["graph_pairs"][k] is None else on(fs["graph_pairs"][k])) for k in ("image", "text")}
+        same = lambda a, b: (a is None and b is None) or (a is not None and b is not None and all(
+            x.shape == y.shape and bool(torch.equal(x, y)) for x, y in zip(a, b)))
+        if not all(same(want[k], self.graph_pairs[k]) for k in ("image", "text")):
+            g = list(self.hs.graphs)
+            for j, key in ((2, "image"), (4, "text")):
+                if want[key] is None:                    # the training graphs, as at step 0 (main.py:68-69)
+                    g[j], g[j + 1] = g[0], g[1]
+                else:
+                    g[j], g[j + 1] = graphs_from_pairs(want[key][0], want[key][1], self.U, self.I)
+            self.hs.graphs = tuple(g)
+            self.graph_pairs = want
+            self._graph = None
+        if hasattr(self.K, "refresh_weight_splits"):     # the bf16 splits of D's weights are cached (DESIGN section 9)
+            self.K.refresh_weight_splits()
 
     # -------------------------------------------------------------- CUDA graph of the steady state
     _graph = None
@@ -244,16 +288,22 @@ class FullStep:
         empty = not self.pairs["image"] and not self.pairs["text"] and all(g.nnz == 0 for g in self.hs.graphs[2:])
         return empty and (rebuild or self.k == 0)
 
-    def capture(self) -> None:
+    def capture(self, keep_state: bool = False) -> None:
         """Capture one steady-state iteration (D step + G step + both optimisers, ~150 launches) into a CUDA graph; ``step``
         replays it whenever ``steady()`` holds and runs eagerly otherwise (first iterations of an epoch).  The random draws
         are static input buffers refilled before every replay (by torch's generator, or by the caller's injected draws).
         Green on the H100 (tests/test_gpu_zzz_gemm_wide.py::test_full_step_cuda_graph_replay_equals_eager).
         NOTE: the warm-up below is ONE REAL iteration on the indices currently in ``hs.idx`` with draws from torch's generator
         (both optimisers step, BatchNorm statistics move): call it where an iteration of the run belongs (trainer.py does), not
-        in front of one."""
+        in front of one.  ``keep_state=True`` undoes it instead: the parameters, both optimisers, BatchNorm statistics, counters
+        and torch's generators are put back as they were before the capture (a resumed run whose saved run had already captured
+        re-captures this way, so it does not train one iteration more than the uninterrupted run)."""
+        from . import checkpoint
         if not self.steady():
             raise RuntimeError("capture() needs the steady state: run the first iterations of the epoch eagerly")
+        dev = self.gsim.device
+        if keep_state:
+            snap, rng = checkpoint.clone_state(self.state_dict()), checkpoint.rng_state(dev)
         self._static = self._draws(None, None, None, None, None)
 
         def warm():
@@ -267,3 +317,6 @@ class FullStep:
             return out
 
         self._graph, self._static_out = capture_graph(warm, body)
+        if keep_state:                  # in place: the captured graph reads the same buffers (the modality graphs did not change)
+            self.load_state_dict(snap)
+            checkpoint.set_rng_state(rng, dev)

@@ -54,6 +54,23 @@ class DiscriminatorState:
     def state_dict(self) -> Dict[str, torch.Tensor]:
         return dict(self.t)
 
+    def optim_state_dict(self) -> Dict[str, object]:
+        """Adam state of ``optim_D``: moments and the step count (host and device copies are the same number)."""
+        return dict(m=dict(self.m), v=dict(self.v), step=int(self.step), step_dev=int(self.step_dev.cpu()[0]))
+
+    def load_state_dict(self, state: Dict[str, torch.Tensor], optim: Optional[Dict[str, object]] = None) -> None:
+        """Copies a ``Discriminator`` state_dict (and, when given, ``optim_state_dict()``) into the live tensors in place.
+        Callers that use the tensor-core GEMM route refresh the cached weight splits afterwards (gan_ops.refresh_weight_splits)."""
+        from .checkpoint import copy_into
+        if optim is not None and int(optim["step"]) != int(optim["step_dev"]):
+            raise ValueError(f"checkpoint mismatch in D step: host {optim['step']}, device {optim['step_dev']}")
+        copy_into(self.t, state, "D")
+        if optim is not None:
+            copy_into(self.m, optim["m"], "D_optim.m")
+            copy_into(self.v, optim["v"], "D_optim.v")
+            self.step = int(optim["step"])
+            self.step_dev.fill_(self.step)
+
     def zeros_like_params(self) -> Dict[str, torch.Tensor]:
         return {k: torch.zeros_like(self.t[k]) for k in PARAMS}
 

@@ -17,7 +17,7 @@ from typing import Dict, Optional, Sequence
 import torch
 import torch.nn.functional as F
 
-from . import ops
+from . import checkpoint, ops
 from .engine import LIVE, P_EI, P_EU, Engine, FeatureStore, capture_graph, join
 from .graph import BipartiteGraph
 
@@ -159,6 +159,33 @@ class HotStep:
             raise RuntimeError("call capture() first")
         self._graph.replay()
         return self.out5
+
+    # ------------------------------------------------------------------ checkpoint (checkpoint.py)
+    _fingerprint = None
+
+    def meta(self) -> dict:
+        if self._fingerprint is None:        # the training graph (graphs[0]) never changes: one device->host copy per step object
+            self._fingerprint = checkpoint.graph_fingerprint(self.graphs[0])
+        m = checkpoint.make_meta(self.U, self.I, self.cfg, self.batch, self.feats, self._fingerprint)
+        if self.sampler is not None:         # with (seed, step_dev) the device sampler's batches are fixed
+            m["sampler_seed"] = int(self.sampler.seed)
+        return m
+
+    def state_dict(self) -> dict:
+        """Parameters (reference keys), AdamW moments and step counter.  Tensors are the live buffers, not copies."""
+        return dict(format=checkpoint.FORMAT, kind="hotstep", meta=self.meta(), model=dict(self.P),
+                    optim=dict(m=dict(self.m), v=dict(self.v), step=int(self.step_dev.cpu()[0])))
+
+    def load_state_dict(self, state: dict) -> None:
+        """Copies a checkpoint (this step's, a FullStep's / Trainer's, or a row-sharded one read at world 1) into the live
+        buffers in place: a graph captured before the load replays from the loaded state."""
+        checkpoint.check_format(state, ("hotstep", "fullstep", "trainer"))
+        checkpoint.check_meta(state["meta"], self.meta())
+        model = {k: state["model"][k] for k in LIVE if k in state["model"]}
+        checkpoint.copy_into(self.P, model, "model")
+        checkpoint.copy_into(self.m, state["optim"]["m"], "optim.m")
+        checkpoint.copy_into(self.v, state["optim"]["v"], "optim.v")
+        self.step_dev.fill_(int(state["optim"]["step"]))
 
     def set_indices(self, users, pos, neg) -> None:
         """Device-side copy of one batch of triples into the static index buffer."""

@@ -26,7 +26,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import _lib, ops
+from . import _lib, checkpoint, ops
 from ._lib import ptr, stream
 from .engine import LIVE, P_EI, P_EU, Engine, FeatureStore, capture_graph
 from .graph import SparseOperand
@@ -449,6 +449,54 @@ class RowShardedHotStep:
             ops.adamw([self.P[k] for k in keys], [self.grads[k] for k in keys], [self.m[k] for k in keys], [self.v[k] for k in keys],
                       self.step_dev, cfg.lr, cfg.beta1, cfg.beta2, cfg.eps, cfg.weight_decay)
         return self.out5
+
+    # -------------------------------------------------------------- checkpoint (checkpoint.py)
+    def meta(self) -> dict:
+        """Same fields as HotStep.meta; the training-matrix fingerprint is summed over the ranks' row blocks (a collective on the
+        first call; the training graph never changes, so it is kept)."""
+        if self._fingerprint is None:
+            ulo, _ = self.pu.bounds(self.rank)
+            nnz, h = checkpoint.graph_fingerprint(self.graphs[0], row0=ulo)
+            if self.pu.world > 1:    # 16-bit limbs: the sum over the ranks cannot overflow int64; recombined mod 2^64 below
+                t = torch.tensor([(h >> (16 * j)) & 0xFFFF for j in range(4)] + [nnz], dtype=torch.int64, device=self.idx.device)
+                dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+                v = [int(x) for x in t.cpu()]
+                h, nnz = sum(v[j] << (16 * j) for j in range(4)) & ((1 << 64) - 1), v[4]
+            self._fingerprint = (nnz, h)
+        return checkpoint.make_meta(self.pu.n, self.pi.n, self.cfg, self.batch, self.feats, self._fingerprint)
+
+    _fingerprint = None
+
+    def state_dict(self) -> dict:
+        """This rank's file of a row-sharded checkpoint (every rank calls it: the fingerprint is a collective): the REAL rows of
+        the rank's blocks of the two tables and of their moments (padding dropped, global row ranges in ``rows``); rank 0 also
+        holds the replicated parameters, their moments and the step counter."""
+        (ulo, uhi), (ilo, ihi) = self.pu.bounds(self.rank), self.pi.bounds(self.rank)
+        rows = {P_EU: uhi - ulo, P_EI: ihi - ilo}
+        keys = [k for k in LIVE if k in rows or self.rank == 0]
+        pick = lambda d: {k: (d[k][:rows[k]] if k in rows else d[k]) for k in keys}
+        return dict(format=checkpoint.FORMAT, kind="rowshard", meta=self.meta(), rows={"user": (ulo, uhi), "item": (ilo, ihi)},
+                    model=pick(self.P), optim=dict(m=pick(self.m), v=pick(self.v), step=int(self.step_dev.cpu()[0])))
+
+    def load_state_dict(self, state: dict) -> None:
+        """Copies ``checkpoint.read_sharded(directory, world, rank)`` of this rank into the live buffers in place."""
+        checkpoint.check_format(state, ("rowshard", "hotstep"))
+        checkpoint.check_meta(state["meta"], self.meta())
+        want = {"user": self.pu.bounds(self.rank), "item": self.pi.bounds(self.rank)}
+        if {k: tuple(v) for k, v in state.get("rows", want).items()} != want:
+            raise ValueError(f"checkpoint mismatch in rows: saved {state['rows']}, this rank {want}")
+        checkpoint.copy_into(self.P, state["model"], "model")
+        checkpoint.copy_into(self.m, state["optim"]["m"], "optim.m")
+        checkpoint.copy_into(self.v, state["optim"]["v"], "optim.v")
+        self.step_dev.fill_(int(state["optim"]["step"]))
+
+    def save(self, directory: str) -> None:
+        """Collective: every rank writes its file of the checkpoint into ``directory``."""
+        checkpoint.save_sharded(self, directory)
+
+    def load(self, directory: str) -> None:
+        """Collective: every rank reads the rows of its blocks from a checkpoint written at any world size."""
+        self.load_state_dict(checkpoint.read_sharded(directory, self.pu.world, self.rank))
 
     # -------------------------------------------------------------- CUDA graph
     def capture(self, warmup: int = 2) -> None:

@@ -28,7 +28,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import gan
+from . import checkpoint, gan
 from .dataset import ReferenceDataset
 from .engine import LIVE
 from .evaluate import Evaluator
@@ -71,6 +71,7 @@ class TrainerArgs:
     feat_reg_decay: float = 1e-5        # :29
     mess_dropout: str = "[0.1, 0.1]"    # :13
     test_flag: str = "part"             # :16
+    checkpoint: str = ""                # not in the reference: train() writes Trainer.save(checkpoint) after every epoch when set
 
 
 def set_seed(seed: int) -> None:
@@ -179,12 +180,58 @@ class Trainer:
             return self._triples[0], self._triples[1], self._triples[2]
         return reference_sample(self.data, self.batch_size, n_items=self.n_items)
 
+    # ------------------------------------------------------------------ checkpoint (checkpoint.py)
+    _loop: Optional[Dict[str, object]] = None        # epoch-loop state after the last finished epoch (what save() writes)
+    _resume: Optional[Dict[str, object]] = None      # set by load(): where the next train() starts
+    _capture_keeps_state = False                     # set by load(): see FullStep.capture(keep_state)
+
+    def save(self, path: str) -> None:
+        """Writes the whole training state at an epoch boundary: the model and the Discriminator under the reference's
+        state_dict keys, both optimisers, the full step's epoch bookkeeping, the epoch loop's state, the sampler position and
+        the RNG states.  ``load`` + ``train()`` continue the run at the next epoch."""
+        st = self.step.state_dict()
+        loop = dict(self._loop or dict(epoch=0, best_recall=0.0, stopping_step=0, test_ret=None, history=[], stopped=False))
+        if loop["test_ret"] is not None:       # the evaluator's numpy arrays travel as tensors (the file loads with weights_only)
+            loop["test_ret"] = {k: torch.from_numpy(v) if isinstance(v, np.ndarray) else v for k, v in loop["test_ret"].items()}
+        st.update(kind="trainer", model=self.model.state_dict(), D=self.D.state_dict(),
+                  trainer=dict(loop=loop, sampler=self.sampler, n_sampled=int(self._n_sampled), rng=checkpoint.rng_state(self.device),
+                               sampler_seed=int(self._dev_sampler.seed) if self.sampler == "device" else None,
+                               captured=self.step._graph is not None))
+        checkpoint.save(st, path)
+
+    def load(self, path: str) -> None:
+        """Restores ``save(path)`` into this Trainer (built with the same data and shape arguments) in place."""
+        st = checkpoint.load(path, kinds=("trainer",))
+        checkpoint.check_meta(st["meta"], self.step.hs.meta())
+        tr = st["trainer"]
+        if tr["sampler"] != self.sampler:
+            raise ValueError(f"checkpoint mismatch in sampler: saved {tr['sampler']!r}, this run {self.sampler!r}")
+        if self.sampler == "device" and tr["sampler_seed"] != self._dev_sampler.seed:     # (seed, step) fixes the batches
+            raise ValueError(f"checkpoint mismatch in sampler_seed: saved {tr['sampler_seed']}, this run {self._dev_sampler.seed}")
+        self.model.load_state_dict(st["model"])          # in place: the unused registered parameters; the live ones and D below
+        self.step.load_state_dict(st)
+        self._n_sampled = int(tr["n_sampled"])
+        loop = dict(tr["loop"])
+        if loop["test_ret"] is not None:
+            loop["test_ret"] = {k: v.numpy() if isinstance(v, torch.Tensor) else v for k, v in loop["test_ret"].items()}
+        self._loop = self._resume = loop
+        self.history = list(loop["history"])
+        # the saved run had captured its steady-state iteration (the capture's warm-up iteration is part of the saved state): the
+        # capture this run makes again must not train one more iteration
+        self._capture_keeps_state = bool(tr["captured"])
+        checkpoint.set_rng_state(tr["rng"], self.device)
+
     # ------------------------------------------------------------------ main.py:308-498
     def train(self) -> Tuple[float, Optional[Dict[str, object]]]:
+        """The epoch loop.  On a Trainer restored by ``load`` it continues at the epoch after the saved one, with the saved
+        best recall, early-stopping count and history."""
         args, data = self.args, self.data
-        stopping_step, best_recall, test_ret = 0, 0.0, None
-        self.history: List[Dict[str, float]] = []
-        for epoch in range(args.epoch):
+        loop = self._resume or dict(epoch=0, best_recall=0.0, stopping_step=0, test_ret=None, history=[], stopped=False)
+        self._resume = None
+        stopping_step, best_recall, test_ret = loop["stopping_step"], loop["best_recall"], loop["test_ret"]
+        self.history: List[Dict[str, float]] = list(loop["history"])
+        ckpt_path = getattr(args, "checkpoint", "")     # a reference parse_args() Namespace has no such flag
+        for epoch in range(loop["epoch"], 0 if loop["stopped"] else args.epoch):
             t1 = time()
             n_batch = data.n_train // args.batch_size + 1                                      # main.py:328
             acc = torch.zeros(4, dtype=torch.float32, device=self.device)                      # loss, mf, emb, cl
@@ -192,7 +239,7 @@ class Trainer:
             for _ in range(n_batch):
                 users, pos, neg = self.sample()
                 if self.cuda_graph and self.step._graph is None and self.step.steady():
-                    self.step.capture()
+                    self.step.capture(keep_state=self._capture_keeps_state)
                 out = self.step.step(users, pos, neg)
                 acc[0] += out["batch_loss"].reshape(())
                 acc[1:3] += out["loss5"][1:3]
@@ -209,6 +256,7 @@ class Trainer:
                                                                                         reg_loss, 0.0))
                 self.last_cl_loss = cl_loss
             t2 = time()
+            stopped = False
             ret = self.test(list(data.val_set.keys()), is_val=True)                            # main.py:451-452 (every epoch)
             t3 = time()
             self.history.append(dict(epoch=epoch, loss=loss, mf_loss=mf_loss, emb_loss=emb_loss, recall=float(ret["recall"][1]),
@@ -230,6 +278,12 @@ class Trainer:
                 self.log("#####Early stopping steps: %d #####" % stopping_step)
             else:
                 self.log("#####Early stop! #####")
+                stopped = True
+            self._loop = dict(epoch=epoch + 1, best_recall=best_recall, stopping_step=stopping_step, test_ret=test_ret,
+                              history=list(self.history), stopped=stopped)
+            if ckpt_path:
+                self.save(ckpt_path)
+            if stopped:
                 break
         self.log(str(test_ret))
         return best_recall, test_ret
