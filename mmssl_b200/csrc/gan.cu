@@ -70,23 +70,27 @@ __global__ void __launch_bounds__(kCT* kRL) bn_fwd_kernel(const float* __restric
     __shared__ float sh[kRL][kCT];
     const int64_t col = (int64_t)blockIdx.x * kCT + threadIdx.x;
     const bool ok = col < h;
+    // The column is summed shifted by its row-0 value k0: a column whose mean is far above its spread loses no digits to the
+    // running sum (fp32 sums of 1e3-sized values are off by far more than the spread's last bits), and a constant column
+    // gives exactly zero deviations, var = 0.
+    const float k0 = ok ? a[col] : 0.f;
     float s = 0.f;
-    if (ok) for (int64_t r = threadIdx.y; r < n; r += kRL) s += a[r * h + col];
-    const float mu = col_reduce(s, sh) / (float)n;
+    if (ok) for (int64_t r = threadIdx.y; r < n; r += kRL) s += a[r * h + col] - k0;
+    const float ms = col_reduce(s, sh) / (float)n;                   // mean - k0
     s = 0.f;
-    if (ok) for (int64_t r = threadIdx.y; r < n; r += kRL) { const float d = a[r * h + col] - mu; s = fmaf(d, d, s); }
+    if (ok) for (int64_t r = threadIdx.y; r < n; r += kRL) { const float d = (a[r * h + col] - k0) - ms; s = fmaf(d, d, s); }
     const float var = col_reduce(s, sh) / (float)n;
     const float rs = 1.0f / sqrtf(var + kBnEps);
     if (!ok) return;
     const float g = gamma[col], b = beta[col];
     for (int64_t r = threadIdx.y; r < n; r += kRL) {
-        const float x = (a[r * h + col] - mu) * rs;
+        const float x = ((a[r * h + col] - k0) - ms) * rs;
         ah[r * h + col] = x;
         hout[r * h + col] = fmaf(x, g, b) * mask[r * h + col];
     }
     if (threadIdx.y == 0) {
         rout[col] = rs;
-        rmean[col] = (1.f - kBnMomentum) * rmean[col] + kBnMomentum * (mu + bias[col]);
+        rmean[col] = (1.f - kBnMomentum) * rmean[col] + kBnMomentum * ((k0 + ms) + bias[col]);
         rvar[col] = (1.f - kBnMomentum) * rvar[col] + kBnMomentum * var * ((float)n / (float)(n - 1));
     }
 }
@@ -298,7 +302,8 @@ __global__ void __launch_bounds__(256) vec_sum_kernel(const float* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------------ CTA-per-row ops
-// gbar = (2 lam / n) (norm - 1) / norm * gx ; sq[row] = (norm - 1)^2
+// gbar = (2 lam / n) (norm - 1) / norm * gx ; sq[row] = (norm - 1)^2.  A row with norm 0 (every head of the batch saturated
+// in fp32, so d out / d x is exactly 0) gets torch's norm backward: a zero gradient, not (-inf) * 0 = NaN; it still adds 1 to sq.
 __global__ void __launch_bounds__(256) gp_rows_kernel(const float* __restrict__ gx, int64_t n, int64_t w, float lam,
                                                       float* __restrict__ gbar, float* __restrict__ sq) {
     __shared__ float sh[33];
@@ -306,7 +311,7 @@ __global__ void __launch_bounds__(256) gp_rows_kernel(const float* __restrict__ 
     float t = 0.f;
     for (int64_t c = threadIdx.x; c < w; c += 256) { const float v = gx[row * w + c]; t = fmaf(v, v, t); }
     const float norm = sqrtf(block_sum_all(t, sh));
-    const float f = (2.f * lam / (float)n) * (norm - 1.f) / norm;
+    const float f = norm > 0.f ? (2.f * lam / (float)n) * (norm - 1.f) / norm : 0.f;
     for (int64_t c = threadIdx.x; c < w; c += 256) gbar[row * w + c] = f * gx[row * w + c];
     if (threadIdx.x == 0) sq[row] = (norm - 1.f) * (norm - 1.f);
 }

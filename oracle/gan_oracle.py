@@ -119,6 +119,41 @@ def real_rows(users, train_csr: sp.csr_matrix, uniform: torch.Tensor, ui_sim: to
     return F.normalize(u_ui, dim=1)
 
 
+def d_step_grads(S, inputf: torch.Tensor, inputr: torch.Tensor, alpha: torch.Tensor, masks1, masks2, cfg: GanConfig):
+    """loss_D of main.py:343-358 and its gradients by autograd, without the optimiser step, in the dtype of S's parameters.
+    inputf / inputr: [2B, I] fake and real rows; alpha [2B] or [2B, 1]; masks1/masks2: the masks of the fake, real and
+    penalty calls.  S is not modified.  Returns gp, the per-row outputs of the three calls, and a gradient per D parameter
+    (zeros where autograd has none: net.8.bias does not reach the penalty)."""
+    Sa = {k: (v.detach().clone().requires_grad_(True) if k in D_PARAMS else v.clone()) for k, v in S.items()}
+    dt = Sa["net.0.weight"].dtype
+    inputf, inputr, alpha = inputf.detach().to(dt), inputr.detach().to(dt), alpha.detach().to(dt).view(-1, 1)
+    masks1, masks2 = [m.to(dt) for m in masks1], [m.to(dt) for m in masks2]
+    outf = discriminator(inputf, Sa, masks1[0], masks2[0])
+    outr = discriminator(inputr, Sa, masks1[1], masks2[1])
+    a = alpha.expand_as(inputr)
+    inter = (a * inputr + (1 - a) * inputf).requires_grad_()
+    outi = discriminator(inter, Sa, masks1[2], masks2[2])
+    gi = autograd.grad(outputs=outi, inputs=inter, grad_outputs=torch.ones_like(outi), create_graph=True, retain_graph=True,
+                       only_inputs=True)[0]
+    gp = ((gi.norm(2, dim=1) - 1) ** 2).mean() * cfg.gp_lambda
+    loss = -outr.mean() + outf.mean() + cfg.gp_rate * gp
+    grads = autograd.grad(loss, [Sa[k] for k in D_PARAMS], allow_unused=True)
+    return dict(gp=gp.detach(), outs=(outf.detach(), outr.detach(), outi.detach()),
+                grads={k: (g.detach() if g is not None else torch.zeros_like(Sa[k])) for k, g in zip(D_PARAMS, grads)})
+
+
+def g_side_grads(S, x_image: torch.Tensor, x_text: torch.Tensor, mask1, mask2, cfg: GanConfig):
+    """The G_rate * G_lossf term of main.py:414-420 on fixed rows: the D outputs and the gradients w.r.t. the image and the
+    text rows, by autograd in the dtype of S's parameters.  S is not modified."""
+    Sa = {k: v.detach().clone() for k, v in S.items()}
+    dt = Sa["net.0.weight"].dtype
+    B = x_image.shape[0]
+    x = torch.cat((x_image.detach(), x_text.detach()), dim=0).to(dt).requires_grad_()
+    out = discriminator(x, Sa, mask1.to(dt), mask2.to(dt))
+    dx = autograd.grad(cfg.G_rate * -out.mean(), x)[0]
+    return out.detach(), dx[:B], dx[B:]
+
+
 def adam_step(p, g, m, v, step: int, lr: float, b1: float = 0.5, b2: float = 0.9, eps: float = 1e-8):
     """torch.optim.Adam (no weight decay), in place; main.py:74."""
     m.mul_(b1).add_(g, alpha=1 - b1)
@@ -136,10 +171,13 @@ def topk_pairs(users, sim: torch.Tensor, n_items: int, cfg: GanConfig) -> Tuple[
     return x, ids.reshape(-1).tolist()
 
 
-def rebuild_graphs(x: List[int], y: List[int], n_users: int, n_items: int) -> Tuple[torch.Tensor, torch.Tensor]:
-    """main.py:379-391 for one modality: (ui, iu) torch sparse graphs from the collected pairs."""
-    tmp = sp.csr_matrix((np.ones(len(x), np.float32), (x, y)), shape=(n_users, n_items))
-    return O.to_torch_coo(O.csr_norm(tmp, True)), O.to_torch_coo(O.csr_norm(tmp.T, True))
+def rebuild_graphs(x: List[int], y: List[int], n_users: int, n_items: int,
+                   dtype=torch.float32) -> Tuple[torch.Tensor, torch.Tensor]:
+    """main.py:379-391 for one modality: (ui, iu) torch sparse graphs from the collected pairs (fp32 like the reference;
+    float64 for a high-precision evaluation)."""
+    vdt = np.float64 if dtype == torch.float64 else np.float32
+    tmp = sp.csr_matrix((np.ones(len(x), vdt), (x, y)), shape=(n_users, n_items))
+    return O.to_torch_coo(O.csr_norm(tmp, True), dtype), O.to_torch_coo(O.csr_norm(tmp.T, True), dtype)
 
 
 # ------------------------------------------------------------------------------------------ the full step
@@ -147,14 +185,20 @@ class FullStep:
     """State + one `step()` = the body of the reference's batch loop (main.py:333-434) with every random draw injected."""
 
     def __init__(self, params: Dict[str, torch.Tensor], d_state: Dict[str, torch.Tensor], image_feats, text_feats,
-                 train_csr: sp.csr_matrix, cfg: O.HotPathConfig, gcfg: GanConfig):
-        self.P = {k: v.clone() for k, v in params.items()}
-        self.S = {k: v.clone() for k, v in d_state.items()}
-        self.feats = (image_feats, text_feats)
-        self.R = train_csr.tocsr()
+                 train_csr: sp.csr_matrix, cfg: O.HotPathConfig, gcfg: GanConfig, dtype=torch.float32):
+        """dtype: float32 (the reference's arithmetic) takes the inputs as given; float64 casts every floating-point input,
+        state and graph, and is the yardstick the device's fp32 results are measured against.  The random draws passed to
+        `step` are cast the same way."""
+        wide = dtype != torch.float32
+        cast = lambda v: v.to(dtype) if wide and v.is_floating_point() else v
+        self.dtype = dtype
+        self.P = {k: cast(v).clone() for k, v in params.items()}
+        self.S = {k: cast(v).clone() for k, v in d_state.items()}
+        self.feats = (cast(image_feats), cast(text_feats))
+        self.R = train_csr.tocsr().astype(np.float64) if wide else train_csr.tocsr()
         self.U, self.I = self.R.shape
         self.cfg, self.g = cfg, gcfg
-        ui, iu = O.build_graphs(self.R)
+        ui, iu = O.build_graphs(self.R, dtype)
         self.graphs = [ui, iu, ui, iu, ui, iu]
         self.idx = 0
         self.index = {"image": ([], []), "text": ([], [])}
@@ -170,6 +214,10 @@ class FullStep:
     def step(self, users, pos, neg, model_masks, d_masks1, d_masks2, gumbel_u, alpha) -> Dict[str, object]:
         """model_masks: 4 [I,d] masks (2 per forward); d_masks1/2: 4 masks each (one per D call); returns a trace dict."""
         cfg, g, B = self.cfg, self.g, self.cfg.batch_size
+        if self.dtype != torch.float32:
+            c = lambda v: v.to(self.dtype)
+            model_masks, d_masks1, d_masks2 = ([c(m) for m in ms] for ms in (model_masks, d_masks1, d_masks2))
+            gumbel_u, alpha = c(gumbel_u), c(alpha)
         tr: Dict[str, object] = {"D_in": [], "D_out": [], "u_sim": []}
         users = [int(u) for u in users]
 
@@ -223,8 +271,8 @@ class FullStep:
         g_img = usim(outs[4], outs[2])
         g_txt = usim(outs[5], outs[3])
         if self.idx % g.T == 0 and self.idx != 0:          # main.py:378-394
-            gi_ui, gi_iu = rebuild_graphs(*self.index["image"], self.U, self.I)
-            gt_ui, gt_iu = rebuild_graphs(*self.index["text"], self.U, self.I)
+            gi_ui, gi_iu = rebuild_graphs(*self.index["image"], self.U, self.I, self.dtype)
+            gt_ui, gt_iu = rebuild_graphs(*self.index["text"], self.U, self.I, self.dtype)
             tr["graphs"] = [gi_ui, gt_ui, gi_iu, gt_iu]     # order of the reference's four conversions
             new_graphs = [self.graphs[0], self.graphs[1], gi_ui, gi_iu, gt_ui, gt_iu]
             self.index = {"image": ([], []), "text": ([], [])}
@@ -316,7 +364,8 @@ def gradient_penalty_closed(x: torch.Tensor, S: Dict[str, torch.Tensor], m1, m2,
     _, gx, k = d_backward(c, S, torch.ones(n), need_dx=True)
     norm = gx.norm(2, dim=1, keepdim=True)
     gp = lam * ((norm - 1) ** 2).mean()
-    gbar = (2 * lam / n) * (norm - 1) * gx / norm                                # d gp / d g     [n, I]
+    # d gp / d g  [n, I]; a zero row (saturated heads) gets torch's norm backward: 0, where the plain formula gives NaN
+    gbar = torch.where(norm > 0, (2 * lam / n) * (norm - 1) / norm, torch.zeros_like(norm)) * gx
     G = {kk: torch.zeros_like(S[kk]) for kk in D_PARAMS}
 
     # ---- reverse of the first-order backward sweep (bottom-up: layer 1 first) ----

@@ -80,18 +80,19 @@ def csr_norm(mat: sp.spmatrix, mean_flag: bool = True) -> sp.spmatrix:
     return left * mat * sp.diags(cs)
 
 
-def to_torch_coo(mat: sp.spmatrix) -> torch.Tensor:
-    """scipy -> torch sparse COO fp32 with int64 indices (main.py:105-112)."""
+def to_torch_coo(mat: sp.spmatrix, dtype=torch.float32) -> torch.Tensor:
+    """scipy -> torch sparse COO with int64 indices (main.py:105-112); fp32 like the reference, float64 for the
+    high-precision evaluations of the tests."""
     coo = mat.tocoo()
     idx = torch.from_numpy(np.vstack((coo.row, coo.col)).astype(np.int64))
     val = torch.from_numpy(np.asarray(coo.data))
-    return torch.sparse_coo_tensor(idx, val, torch.Size(coo.shape)).to(torch.float32)
+    return torch.sparse_coo_tensor(idx, val, torch.Size(coo.shape)).to(dtype)
 
 
-def build_graphs(train_mat: sp.spmatrix) -> Tuple[torch.Tensor, torch.Tensor]:
+def build_graphs(train_mat: sp.spmatrix, dtype=torch.float32) -> Tuple[torch.Tensor, torch.Tensor]:
     """ui_graph, iu_graph as Trainer.__init__ builds them (main.py:58,65-67)."""
-    ui = to_torch_coo(csr_norm(train_mat, mean_flag=True))
-    iu = to_torch_coo(csr_norm(train_mat.T, mean_flag=True))
+    ui = to_torch_coo(csr_norm(train_mat, mean_flag=True), dtype)
+    iu = to_torch_coo(csr_norm(train_mat.T, mean_flag=True), dtype)
     return ui, iu
 
 

@@ -66,10 +66,12 @@ def head_bwd(s, coef, w3, h2):
 
 
 def gp_rows(gx, lam):
+    """A row with norm 0 gets a zero gradient, as torch's norm backward gives it (and still adds (0 - 1)^2 to gp)."""
     n = gx.shape[0]
     norm = gx.norm(2, dim=1, keepdim=True)
     gp = lam * ((norm - 1) ** 2).mean()
-    return gp.view(1), (2 * lam / n) * (norm - 1) * gx / norm
+    f = torch.where(norm > 0, (2 * lam / n) * (norm - 1) / norm, torch.zeros_like(norm))
+    return gp.view(1), f * gx
 
 
 def gp_rev_bn(q, dy, ah, r, gamma, mask):

@@ -160,6 +160,97 @@ def test_closed_form_gradient_penalty_matches_double_backward():
             assert rel_err(G[k].view_as(w), w) < 1e-9, k
 
 
+def test_closed_form_gradient_penalty_with_saturated_heads():
+    """Every head saturated (sigmoid == 1 exactly): d out / d x is exactly zero on every row.  Autograd's norm backward gives
+    such a row a zero gradient, so gp = lambda and every penalty gradient is 0; the closed form must not turn (-inf) * 0
+    into NaN."""
+    S, g = _random_d(seed=5)
+    S["net.8.bias"] = torch.full((1,), 60.0, dtype=torch.float64)      # sigmoid(z) == 1 in float64 for z > 37
+    n, I = 32, 96
+    xr = torch.nn.functional.normalize(torch.rand(n, I, generator=g).double(), dim=1)
+    xf = torch.nn.functional.normalize(torch.randn(n, I, generator=g).double(), dim=1)
+    alpha = torch.rand(n, 1, generator=g).double()
+    m1 = ((torch.rand(n, I // 4, generator=g) >= 0.31) / 0.69).double()
+    m2 = ((torch.rand(n, I // 8, generator=g) >= 0.5) / 0.5).double()
+    Sa = {k: (v.clone().requires_grad_(True) if k in GO.D_PARAMS else v.clone()) for k, v in S.items()}
+    gp_a = GO.gradient_penalty(Sa, xr, xf, alpha, m1, m2, GO.GanConfig())
+    want = torch.autograd.grad(gp_a, [Sa[k] for k in GO.D_PARAMS], allow_unused=True)
+    assert float(gp_a) == 0.3 and all(w is None or float(w.abs().max()) == 0.0 for w in want)
+    gp_c, G = GO.gradient_penalty_closed(alpha * xr + (1 - alpha) * xf, S, m1, m2, lam=0.3)
+    assert float(gp_c) == 0.3
+    for k in GO.D_PARAMS:
+        assert bool(torch.isfinite(G[k]).all()) and float(G[k].abs().max()) == 0.0, k
+
+
+def test_gp_rows_spec_on_zero_and_unit_rows_matches_autograd():
+    """tests/gan_ops_cpu.gp_rows (the kernel's specification) against autograd of lam * mean((||g|| - 1)^2) in float64, on
+    rows of norm 0, rows of norm exactly 1 and rows of 1e-20 next to ordinary rows."""
+    from tests import gan_ops_cpu as REF
+    g = torch.Generator().manual_seed(8)
+    n, w = 10, 7
+    gx = torch.randn(n, w, generator=g, dtype=torch.float64)
+    gx[1] = 0.0
+    gx[4] = 0.0
+    gx[2] = 0.0
+    gx[2, 3] = 1.0                                     # norm exactly 1: zero gradient, zero penalty
+    gx[6] = 1e-20 * torch.randn(w, generator=g, dtype=torch.float64)
+    ga = gx.clone().requires_grad_(True)
+    gp_a = 0.3 * ((ga.norm(2, dim=1) - 1) ** 2).mean()
+    want = torch.autograd.grad(gp_a, ga)[0]
+    gp, gbar = REF.gp_rows(gx, 0.3)
+    assert abs(float(gp) - float(gp_a)) < 1e-15 and bool(torch.isfinite(gbar).all())
+    assert float(gbar[1].abs().max()) == 0.0 and float(gbar[4].abs().max()) == 0.0 and float(gbar[2].abs().max()) == 0.0
+    assert rel_err(gbar, want) < 1e-14
+
+
+def test_float64_full_step_runs_in_float64():
+    """FullStep(dtype=torch.float64) casts state, features, graphs and draws: every recorded result is float64, and one
+    iteration agrees with the fp32 oracle to fp32 accuracy."""
+    from tests import fullstep_check
+    z, c = fullstep_check.load_trace()
+    t = lambda a: torch.from_numpy(np.asarray(a)).clone()
+    R = sp.csr_matrix((np.ones(len(z["train_rows"]), np.float32), (z["train_rows"], z["train_cols"])), shape=(c["U"], c["I"]))
+    cfg = O.HotPathConfig(embed_size=c["d"], n_layers=c["n_layers"], head_num=c["head_num"], id_cat_rate=c["id_cat_rate"],
+                          model_cat_rate=c["model_cat_rate"], drop_rate=c["drop_rate"], tau=c["tau"], cl_rate=c["cl_rate"],
+                          emb_decay=c["emb_decay"], feat_reg_decay=c["feat_reg_decay"], batch_size=c["B"], lr=c["lr"])
+    g = GO.GanConfig(G_rate=c["G_rate"], D_lr=c["D_lr"], gp_rate=c["gp_rate"], m_topk_rate=c["m_topk_rate"], T=c["T"])
+    P = {k[3:]: t(z[k]) for k in z.files if k.startswith("G0/")}
+    S = {k[3:]: t(z[k]) for k in z.files if k.startswith("D0/")}
+    runs = {}
+    for dt in (torch.float32, torch.float64):
+        fs = GO.FullStep(P, S, t(z["image_feats"]), t(z["text_feats"]), R, cfg, g, dtype=dt)
+        users, pos, neg = (z["sample"][0][j] for j in range(3))
+        runs[dt] = fs.step(users, pos, neg, [t(z["mask_model"][j]) for j in range(4)], [t(z["mask_d1"][j]) for j in range(4)],
+                           [t(z["mask_d2"][j]) for j in range(4)], t(z["gumbel_u"][0]), t(z["alpha"][0]))
+    lo, hi = runs[torch.float32], runs[torch.float64]
+    assert hi["gp"].dtype == torch.float64 and all(v.dtype == torch.float64 for v in hi["Ggrad"].values())
+    assert all(x.dtype == torch.float64 for x in hi["u_sim"] + hi["D_out"])
+    assert abs(float(lo["gp"]) - float(hi["gp"])) < 1e-4 * abs(float(hi["gp"]))
+    for k in GO.D_PARAMS:
+        if k not in DEAD_BIAS:
+            assert rel_err(lo["Dgrad"][k], hi["Dgrad"][k]) < 1e-4, k
+    for k in hi["Ggrad"]:
+        assert rel_err(lo["Ggrad"][k], hi["Ggrad"][k]) < 1e-4, k
+
+
+def test_d_step_grads_matches_full_step_trace(replay):
+    """gan_oracle.d_step_grads (the yardstick of the device's composite D step) == the D gradients FullStep records."""
+    z, c, traces = replay
+    S = {k[3:]: torch.from_numpy(np.asarray(z[k])).clone() for k in z.files if k.startswith("D0/")}
+    B = c["B"]
+    tr = traces[0]
+    t = lambda a: torch.from_numpy(np.asarray(a))
+    res = GO.d_step_grads(S, tr["D_in"][0], tr["D_in"][1], t(z["alpha"][0]), [t(z["mask_d1"][j]) for j in range(3)],
+                          [t(z["mask_d2"][j]) for j in range(3)], GO.GanConfig(gp_rate=c["gp_rate"]))
+    assert abs(float(res["gp"]) - float(tr["gp"])) <= 1e-6 * abs(float(tr["gp"]))
+    for j in range(3):
+        assert rel_err(res["outs"][j], tr["D_out"][j]) < 1e-6
+    for k in GO.D_PARAMS:
+        if k not in DEAD_BIAS:
+            assert rel_err(res["grads"][k], tr["Dgrad"][k]) < 1e-6, k
+    assert tr["D_in"][1].shape[0] == 2 * B
+
+
 def test_closed_form_u_sim_backward_matches_autograd():
     g = torch.Generator().manual_seed(2)
     U, I, d, B = 40, 50, 16, 12

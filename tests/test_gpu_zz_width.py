@@ -168,12 +168,15 @@ def test_rejections():
 
 
 def test_full_step_d96_vs_gan_oracle():
-    """One FullStep iteration (D step + G step + both optimisers + graph rebuild) at d = 96 against oracle/gan_oracle.py with the
-    same injected draws.  (With 97 items instead of 101, the Discriminator weight net.4.weight differs from the oracle by 6.3e-4
-    relative, above the 5e-4 bound, identically on the H100 and the emulator; the other item counts tried at d = 96 agree to
-    2e-7.  The cause is not known yet.)"""
+    """One FullStep iteration (D step + G step + both optimisers + graph rebuild) at d = 96 and 97 items against
+    oracle/gan_oracle.py with the same injected draws; the Discriminator by its gradients against float64.  Its weights after
+    Adam are not compared here: at 97 items net.4.weight after Adam differs from the fp32 oracle's by 6.3e-4 while the gradients
+    that produced it are within the float64 bound (fullstep_check.within_fp32_reach) -- Adam's m / (sqrt(v) + eps) in its first
+    step is sign(g) * lr for every entry, so an entry near zero whose sign differs moves by 2 lr (DESIGN sections 2 and 6)."""
     from tests import fullstep_check
-    fullstep_check.random_problem_check("cuda", d=96, I=101, steps=1)
+    _, dist = fullstep_check.random_problem_check("cuda", d=96, I=97, steps=1, d_state_check=False)
+    print("d=96 I=97 D step, distance to float64 (device, fp32 autograd):",
+          {k: ("%.3g" % a, "%.3g" % b) for k, (a, b) in dist.items()})
 
 
 def test_trainer_two_epochs_d32():
