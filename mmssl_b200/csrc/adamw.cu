@@ -17,6 +17,11 @@ struct AdamPack {
     int n;
 };
 
+// 1 - beta^step.  Formed as 1.f - powf(beta, step) it cancels: beta^step near 1 is rounded to 2^-24 of 1, which is 3e-5 of
+// 1 - 0.999^2.  beta - 1 is exact in fp32 (beta in [0.5, 1)) and log1pf / expm1f keep the relative accuracy of a small argument.
+__device__ __forceinline__ float bias_correction(float beta, int step) {
+    return -expm1f((float)step * log1pf(beta - 1.f)); }
+
 __global__ void step_tick_kernel(int32_t* step) {
     pdl_wait(); *step += 1; }
 
@@ -24,8 +29,8 @@ __global__ void __launch_bounds__(256) adamw_kernel(const AdamPack pk, const int
                                                     float b1, float b2, float eps, float wd) {
     pdl_wait();
     const int step = *step_dev;
-    const float bc1 = 1.f - powf(b1, (float)step);
-    const float bc2 = 1.f - powf(b2, (float)step);
+    const float bc1 = bias_correction(b1, step);
+    const float bc2 = bias_correction(b2, step);
     const float step_size = lr / bc1;
     const float inv_sqrt_bc2 = rsqrtf(bc2);
     const float decay = 1.f - lr * wd;
@@ -73,8 +78,8 @@ __global__ void __launch_bounds__(256) dp_fused_adamw_kernel(const float* __rest
                                                              float lr, float b1, float b2, float eps, float wd) {
     // step_dev != NULL: the 1-based step number lives on the device (mmssl_step_tick), so the launch can sit in a CUDA graph
     const int step = step_dev != nullptr ? *step_dev : step_host;
-    const float bc1 = 1.f - powf(b1, (float)step);
-    const float bc2 = 1.f - powf(b2, (float)step);
+    const float bc1 = bias_correction(b1, step);
+    const float bc2 = bias_correction(b2, step);
     const float step_size = lr / bc1;
     const float inv_sqrt_bc2 = rsqrtf(bc2);
     const float decay = 1.f - lr * wd;
