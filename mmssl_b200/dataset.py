@@ -11,14 +11,19 @@
    user rows of A_ui and (A_iu)^T, item rows of A_iu, (A_ui)^T and of the features) without reading the rest: the slices are
    views of the maps (indices / values are contiguous per row block), so a rank touches 1/world of the bytes and the
    host->device copy can run straight from the page cache.
+4. The held-out sets (``val_set`` / ``test_set``) are written beside the operands as CSR over users (``val.*`` / ``test.*``:
+   sorted rows, global item ids, empty rows for users without one); ``ShardedDataset.held`` and ``train_rows`` hand a rank the
+   rows of its user block for the sharded evaluator (evaluate.ShardedEvaluator).  A directory written before they existed
+   still opens and trains; only ``held`` needs them.
 """
 from __future__ import annotations
 
+import itertools
 import json
 import os
 import pickle
 from dataclasses import dataclass, field
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 import scipy.sparse as sp
@@ -28,6 +33,7 @@ from .synthetic import csr_norm
 
 OPERANDS = ("ui", "iu", "iuT", "uiT")       # A_ui [U,I], A_iu [I,U], (A_iu)^T [U,I], (A_ui)^T [I,U]
 ROW_SPACE = {"ui": "user", "iuT": "user", "iu": "item", "uiT": "item"}
+HELD = ("val", "test")                      # held-out sets, CSR over users (meta.json "held")
 
 
 @dataclass
@@ -83,6 +89,20 @@ def _write(path: str, arr: np.ndarray, dtype) -> None:
     np.ascontiguousarray(arr, dtype=np.dtype(dtype).newbyteorder("<")).tofile(path)
 
 
+def held_csr(rows: Dict[int, List[int]], n_rows: int) -> Tuple[np.ndarray, np.ndarray]:
+    """dict user -> item list -> CSR (indptr int64 [n_rows + 1], indices int64) with every row sorted and duplicate ids kept,
+    the rows ``evaluate.Evaluator`` builds from the same dict."""
+    users = np.fromiter((int(u) for u in rows), np.int64, len(rows))
+    if users.size and (users.min() < 0 or users.max() >= n_rows):
+        raise ValueError(f"held-out rows name a user outside [0, {n_rows})")
+    lens = np.fromiter((len(v) for v in rows.values()), np.int64, len(rows))
+    indptr = np.zeros(n_rows + 1, np.int64)
+    indptr[users + 1] = lens
+    np.cumsum(indptr, out=indptr)
+    flat = np.fromiter(itertools.chain.from_iterable(rows.values()), np.int64, int(lens.sum()))
+    return indptr, flat[np.lexsort((flat, np.repeat(users, lens)))]
+
+
 def write_shards(ds: ReferenceDataset, out_dir: str) -> Dict[str, object]:
     """Flat arrays + meta.json.  Independent of the world size: the row blocks are cut at open time."""
     os.makedirs(out_dir, exist_ok=True)
@@ -100,6 +120,12 @@ def write_shards(ds: ReferenceDataset, out_dir: str) -> Dict[str, object]:
         meta["operands"][name] = {"rows": int(m.shape[0]), "cols": int(m.shape[1]), "nnz": int(m.nnz)}
     _write(os.path.join(out_dir, "image_feat.f32"), ds.image_feats, np.float32)
     _write(os.path.join(out_dir, "text_feat.f32"), ds.text_feats, np.float32)
+    meta["held"] = {}
+    for name, rows in (("val", ds.val_set), ("test", ds.test_set)):
+        indptr, indices = held_csr(rows, U)
+        _write(os.path.join(out_dir, f"{name}.indptr.i64"), indptr, np.int64)
+        _write(os.path.join(out_dir, f"{name}.indices.i32"), indices, np.int32)
+        meta["held"][name] = {"rows": int(U), "nnz": int(indices.size)}
     with open(os.path.join(out_dir, "meta.json"), "w") as f:
         json.dump(meta, f, indent=1)
     return meta
@@ -107,16 +133,18 @@ def write_shards(ds: ReferenceDataset, out_dir: str) -> Dict[str, object]:
 
 @dataclass
 class CsrBlock:
-    """Row block [lo, hi) of an operand, padded to `block` rows; indptr is rebased to 0, indices are GLOBAL column ids."""
+    """Row block [lo, hi) of an operand, padded to `block` rows; indptr is rebased to 0, indices are GLOBAL column ids.
+    ``values`` is None for a pattern (held-out rows, training rows): ``to_scipy`` then gives it ones."""
     indptr: np.ndarray
     indices: np.ndarray
-    values: np.ndarray
+    values: Optional[np.ndarray]
     shape: Tuple[int, int]
     lo: int
     hi: int
 
     def to_scipy(self) -> sp.csr_matrix:
-        return sp.csr_matrix((self.values, self.indices, self.indptr), shape=self.shape)
+        vals = self.values if self.values is not None else np.ones(self.indices.size, np.float32)
+        return sp.csr_matrix((vals, self.indices, self.indptr), shape=self.shape)
 
 
 class ShardedDataset:
@@ -136,18 +164,39 @@ class ShardedDataset:
     def _map(self, name: str, dtype, shape=None) -> np.ndarray:
         return np.memmap(os.path.join(self.root, name), dtype=np.dtype(dtype).newbyteorder("<"), mode="r", shape=shape)
 
-    def operand(self, name: str) -> CsrBlock:
-        info = self.meta["operands"][name]
-        part = self.part[ROW_SPACE[name]]
+    def _block(self, name: str, part: RowPartition, rows: int, nnz: int, cols: int, values: bool) -> CsrBlock:
         lo, hi = part.bounds(self.rank)
-        ip = self._map(f"{name}.indptr.i64", np.int64, (info["rows"] + 1,))
+        ip = self._map(f"{name}.indptr.i64", np.int64, (rows + 1,))
         b, e = int(ip[lo]), int(ip[hi])
         indptr = np.empty(part.block + 1, np.int64)
         indptr[:hi - lo + 1] = ip[lo:hi + 1] - b
         indptr[hi - lo + 1:] = e - b                             # padding rows are empty
-        idx = self._map(f"{name}.indices.i32", np.int32, (info["nnz"],))[b:e]
-        val = self._map(f"{name}.values.f32", np.float32, (info["nnz"],))[b:e]
-        return CsrBlock(indptr, idx, val, (part.block, info["cols"]), lo, hi)
+        if nnz == 0:                                             # an empty file cannot be mapped (an empty held-out set)
+            return CsrBlock(indptr, np.zeros(0, np.int32), np.zeros(0, np.float32) if values else None, (part.block, cols), lo, hi)
+        idx = self._map(f"{name}.indices.i32", np.int32, (nnz,))[b:e]
+        val = self._map(f"{name}.values.f32", np.float32, (nnz,))[b:e] if values else None
+        return CsrBlock(indptr, idx, val, (part.block, cols), lo, hi)
+
+    def operand(self, name: str) -> CsrBlock:
+        info = self.meta["operands"][name]
+        return self._block(name, self.part[ROW_SPACE[name]], info["rows"], info["nnz"], info["cols"], True)
+
+    def train_rows(self) -> CsrBlock:
+        """The training items of the rank's user block: the column pattern of its ``ui`` rows (sorted global item ids, no
+        values), i.e. the rows of ``train_mat`` -- the graph the model trains on, and ``Data.train_items`` wherever the
+        dataset's train.json and train_mat agree."""
+        info = self.meta["operands"]["ui"]
+        return self._block("ui", self.part["user"], info["rows"], info["nnz"], info["cols"], False)
+
+    def held(self, split: str) -> CsrBlock:
+        """The held-out items ('val' or 'test') of the rank's user block: sorted global item ids, no values."""
+        if split not in HELD:
+            raise ValueError(f"split must be one of {HELD}, not {split!r}")
+        info = self.meta.get("held", {}).get(split)
+        if info is None:
+            raise ValueError(f"{self.root}: no held-out '{split}' rows ({split}.indptr.i64 / {split}.indices.i32 are missing; "
+                             f"write the directory again with dataset.write_shards)")
+        return self._block(split, self.part["user"], info["rows"], info["nnz"], self.n_items, False)
 
     def features(self, which: str) -> np.ndarray:
         """This rank's item rows of 'image' / 'text' features: a [hi-lo, D] view of the map (no copy)."""

@@ -5,7 +5,9 @@ ranks them in a ``multiprocessing.Pool`` with ``heapq`` (batch_test.py:112-169);
 training items, hit marking and the metrics are one kernel and only the [4, len(Ks)] result leaves the GPU.
 ``test_flag='full'`` (batch_test.py:38-68, 104-107) adds the per-user ROC-AUC over all non-training items
 (``mmssl_eval_rank_full``): the same sweep, no host sort.  Ks is any list of cut-offs >= 1 (parser.py:63), unsorted or with
-duplicates: up to 8 cut-offs of at most 64 go to the shared-memory kernel, any other list to ``mmssl_eval_rank_wide``."""
+duplicates: up to 8 cut-offs of at most 64 go to the shared-memory kernel, any other list to ``mmssl_eval_rank_wide``.
+``ShardedEvaluator`` is the same evaluation for a row-sharded model (rowshard_step.py), on the ranks that hold it, with the
+one-GPU result bit for bit."""
 from __future__ import annotations
 
 import ctypes as C
@@ -13,9 +15,13 @@ from typing import Dict, Mapping, Sequence
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from . import _lib
 from ._lib import ptr, stream
+from .parallel import RowPartition, all_gather_rows
+
+_BAD_USER = "users_to_test holds an id outside [0, n_users): the ranking kernel indexes the CSR row pointers with it"
 
 
 def _rows_to_csr(rows: Mapping[int, Sequence[int]], n_users: int, device) -> tuple:
@@ -39,6 +45,20 @@ class Evaluator:
     def __init__(self, train_items: Mapping[int, Sequence[int]], test_set: Mapping[int, Sequence[int]],
                  val_set: Mapping[int, Sequence[int]], n_users: int, n_items: int, Ks: Sequence[int] = (10, 20, 50), device="cuda",
                  test_flag: str = "part"):
+        self._setup(n_users, n_items, Ks, device, test_flag)
+        self._set_rows(_rows_to_csr(train_items, n_users, self.device), _rows_to_csr(test_set, n_users, self.device),
+                       _rows_to_csr(val_set, n_users, self.device))
+
+    @classmethod
+    def _from_csr(cls, train, test, val, n_users: int, n_items: int, Ks: Sequence[int], device, test_flag: str) -> "Evaluator":
+        """The same evaluator over rows that are already (indptr, indices) int64 tensors on `device`, sorted within each row
+        (ShardedEvaluator: a rank's user block, built from the shard arrays without per-user dicts)."""
+        ev = cls.__new__(cls)
+        ev._setup(n_users, n_items, Ks, device, test_flag)
+        ev._set_rows(train, test, val)
+        return ev
+
+    def _setup(self, n_users, n_items, Ks, device, test_flag) -> None:
         if test_flag not in ("part", "full"):
             raise ValueError(f"test_flag must be 'part' or 'full', not {test_flag!r}")
         self.test_flag = test_flag
@@ -50,8 +70,10 @@ class Evaluator:
         # the kernel with 512-key shared buffers and a 64-bit hit mask takes up to 8 cut-offs of at most 64
         self.wide = len(self.Ks) > 8 or max(self.Ks) > 64
         self.device = torch.device(device)
-        self.train = _rows_to_csr(train_items, n_users, self.device)
-        self.held = {False: _rows_to_csr(test_set, n_users, self.device), True: _rows_to_csr(val_set, n_users, self.device)}
+
+    def _set_rows(self, train, test, val) -> None:
+        self.train = train
+        self.held = {False: test, True: val}
         self._held_len = {k: np.diff(v[0].cpu().numpy()) for k, v in self.held.items()}
         self._ks = (C.c_int32 * len(self.Ks))(*self.Ks)
         self._ks_dev = torch.tensor(self.Ks, dtype=torch.int32).to(self.device) if self.wide else None
@@ -73,7 +95,7 @@ class Evaluator:
             raise ValueError("embedding tables do not match the evaluator's shapes")
         ids = torch.as_tensor(list(users_to_test) if not torch.is_tensor(users_to_test) else users_to_test)
         if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= min(self.n_users, ua.shape[0])):
-            raise ValueError("users_to_test holds an id outside [0, n_users): the ranking kernel indexes the CSR row pointers with it")
+            raise ValueError(_BAD_USER)
         users_np = np.asarray(list(users_to_test), np.int64)
         users = torch.as_tensor(users_np).to(self.device)
         n, kmax, nk, d = users.numel(), max(self.Ks), len(self.Ks), ua.shape[1]
@@ -118,11 +140,155 @@ class Evaluator:
     def test_torch(self, ua_embeddings, ia_embeddings, users_to_test, is_val, drop_flag=False, batch_test_flag=False):
         """Same signature and result as batch_test.py:112-169 ('auc' is 0. in the default test_flag == 'part' mode, the mean
         per-user ROC-AUC in 'full' mode -- NaN as soon as one evaluated user has a single class, like the reference)."""
-        out = self.rank(ua_embeddings, ia_embeddings, users_to_test, is_val)
-        res = out["result"].cpu().numpy()
-        auc = 0.
-        if self.test_flag == "full":
-            mean = torch.zeros(1, dtype=torch.float64, device=self.device)
-            _lib.check(_lib.load().mmssl_eval_reduce(ptr(out["auc"]), out["auc"].numel(), 1, ptr(mean), stream()))
-            auc = float(mean.cpu()[0])
-        return {"precision": res[0].copy(), "recall": res[1].copy(), "ndcg": res[2].copy(), "hit_ratio": res[3].copy(), "auc": auc}
+        return _test_result(self.rank(ua_embeddings, ia_embeddings, users_to_test, is_val), self.test_flag, self.device)
+
+
+def _test_result(out: Dict[str, torch.Tensor], test_flag: str, device) -> Dict[str, object]:
+    """batch_test.py's result dict from rank()'s output: the [4, nK] metrics and, in full mode, the mean of the per-user AUC."""
+    res = out["result"].cpu().numpy()
+    auc = 0.
+    if test_flag == "full":
+        mean = torch.zeros(1, dtype=torch.float64, device=device)
+        _lib.check(_lib.load().mmssl_eval_reduce(ptr(out["auc"]), out["auc"].numel(), 1, ptr(mean), stream()))
+        auc = float(mean.cpu()[0])
+    return {"precision": res[0].copy(), "recall": res[1].copy(), "ndcg": res[2].copy(), "hit_ratio": res[3].copy(), "auc": auc}
+
+
+def _device_csr(indptr, indices, device) -> tuple:
+    """(indptr, indices) host arrays (indices int32 or int64, e.g. views of the shard maps) -> the kernels' int64 tensors; the
+    indices travel as they are and are widened on the device."""
+    ip = torch.from_numpy(np.array(indptr, dtype=np.int64)).to(device)
+    ix = torch.from_numpy(np.array(indices, dtype=np.int32 if np.asarray(indices).dtype.itemsize == 4 else np.int64)).to(device)
+    return ip, ix.to(torch.int64)
+
+
+def _block_rows(rows: Mapping[int, Sequence[int]], part: RowPartition, rank: int) -> tuple:
+    """dict user -> item list -> CSR of the rank's user block (local row ids, sorted rows, padding rows empty)."""
+    from .dataset import held_csr
+    lo, hi = part.bounds(rank)
+    return held_csr({int(u) - lo: its for u, its in rows.items() if lo <= int(u) < hi}, part.block)
+
+
+class ShardedEvaluator:
+    """``Evaluator`` for a model whose tables are row-sharded over the ranks of a process group (rowshard_step.py): one per
+    rank, holding only the train / test / val rows of the rank's user block.
+
+    ``rank(u_local, i_local, users_to_test, is_val)`` takes the rank's padded [block, d] rows of the final user and item tables
+    and the same list of global user ids on every rank, and
+      1. all-gathers the item table (n_items x d fp32 on every rank: 1 GB at 1M items, d = 256);
+      2. ranks the listed users that fall in the rank's block, with local ids against the rank's rows, by the same kernels
+         (``Evaluator.rank``'s launch code; item ids stay global, so the tie rule -- equal score, lower id first -- is the same);
+      3. all-gathers the per-user metric rows (and per-user AUC in full mode), padded to the largest per-rank count, places them
+         at their positions in ``users_to_test`` and runs ``mmssl_eval_reduce`` over the assembled [n, 4, nK] buffer.
+    A per-user row depends only on that user's vector, the item table and the user's rows, and the reduction runs over the rows
+    in list order as on one GPU, so every rank's result (and mean AUC) is bitwise what ``Evaluator`` returns on the gathered
+    tables.  The gathered and the assembled rows take n * (4 nK + 1) * 8 bytes each: about 1 GB at 10M users and three
+    cut-offs.  The ranked lists are not gathered: each rank returns its own, with their positions in ``users_to_test``."""
+
+    _local_cls = Evaluator       # the class itself, bound when this module is imported
+
+    def __init__(self, train, test, val, part_u: RowPartition, part_i: RowPartition, rank: int, n_items: int,
+                 Ks: Sequence[int] = (10, 20, 50), test_flag: str = "part", group=None, device="cuda"):
+        """train / test / val: (indptr, indices) of the rank's user block -- indptr [block + 1] rebased to 0, indices global
+        item ids sorted within each row (int32 or int64)."""
+        if int(n_items) != part_i.n:
+            raise ValueError(f"n_items {n_items} does not match the item partition ({part_i.n} rows)")
+        for name, (ip, _) in (("train", train), ("test", test), ("val", val)):
+            if len(ip) != part_u.block + 1:
+                raise ValueError(f"{name} rows: indptr of {len(ip)} entries, the user block needs {part_u.block + 1}")
+        self.pu, self.pi, self.rank_id, self.group = part_u, part_i, int(rank), group
+        self.n_users, self.n_items = part_u.n, int(n_items)
+        dev = torch.device(device)
+        rows = [_device_csr(ip, ix, dev) for ip, ix in (train, test, val)]
+        self._local = self._local_cls._from_csr(*rows, part_u.block, n_items, Ks, dev, test_flag)
+        self.Ks, self.test_flag, self.wide, self.device = self._local.Ks, test_flag, self._local.wide, dev
+
+    @classmethod
+    def from_shards(cls, sh, Ks: Sequence[int] = (10, 20, 50), test_flag: str = "part", group=None, device="cuda") -> "ShardedEvaluator":
+        """From ``dataset.ShardedDataset`` (rank and world as it was opened with): training rows = the pattern of the rank's ``ui``
+        rows, held-out rows from the ``val`` / ``test`` arrays."""
+        pair = lambda b: (b.indptr, b.indices)
+        return cls(pair(sh.train_rows()), pair(sh.held("test")), pair(sh.held("val")), sh.part["user"], sh.part["item"], sh.rank,
+                   sh.n_items, Ks, test_flag, group, device)
+
+    @classmethod
+    def from_rows(cls, train_items, test_set, val_set, n_users: int, n_items: int, part_u: RowPartition, part_i: RowPartition,
+                  rank: int, Ks: Sequence[int] = (10, 20, 50), test_flag: str = "part", group=None, device="cuda") -> "ShardedEvaluator":
+        """From the reference's dicts (``Data.train_items`` / ``test_set`` / ``val_set``); every rank keeps its block's rows."""
+        if part_u.n != int(n_users):
+            raise ValueError(f"n_users {n_users} does not match the user partition ({part_u.n} rows)")
+        rows = [_block_rows(r, part_u, rank) for r in (train_items, test_set, val_set)]
+        return cls(*rows, part_u, part_i, rank, n_items, Ks, test_flag, group, device)
+
+    # ------------------------------------------------------------------ the phases of rank()
+    def check_users(self, users_to_test) -> np.ndarray:
+        ids = users_to_test.detach().cpu().numpy() if torch.is_tensor(users_to_test) else list(users_to_test)
+        ids = np.asarray(ids, np.int64).reshape(-1)
+        if ids.size and (int(ids.min()) < 0 or int(ids.max()) >= self.n_users):
+            raise ValueError(_BAD_USER)
+        return ids
+
+    def gather_items(self, i_local: torch.Tensor) -> torch.Tensor:
+        """[block, d] item rows of every rank -> the full [n_items, d] table."""
+        return all_gather_rows(i_local.detach(), self.pi, self.group)
+
+    def rank_local(self, u_local: torch.Tensor, items: torch.Tensor, ids: np.ndarray, is_val: bool):
+        """Ranks the entries of `ids` in the rank's user block.  Returns (Evaluator.rank's output, their positions in `ids`)."""
+        lo = self.rank_id * self.pu.block
+        mine = np.nonzero(ids // self.pu.block == self.rank_id)[0]
+        if mine.size == 0:           # none of the listed users is here: no launch (the kernels take no empty outputs)
+            kmax, nk, dev = max(self.Ks), len(self.Ks), self.device
+            out = dict(ranked=torch.empty(0, kmax, dtype=torch.int32, device=dev),
+                       ranked_scores=torch.empty(0, kmax, dtype=torch.float32, device=dev),
+                       hits=torch.empty(0, kmax, dtype=torch.int32, device=dev),
+                       per_user=torch.empty(0, 4, nk, dtype=torch.float64, device=dev))
+            if self.test_flag == "full":
+                out["auc"] = torch.empty(0, dtype=torch.float64, device=dev)
+            return out, mine
+        return self._local.rank(u_local, items, ids[mine] - lo, is_val), mine
+
+    def combine(self, local: Dict[str, torch.Tensor], ids: np.ndarray) -> Dict[str, torch.Tensor]:
+        """Every rank's per-user rows at their positions in `ids`, and the result reduced over them in that order."""
+        nk, n, world, dev = len(self.Ks), ids.size, self.pu.world, self.device
+        full = self.test_flag == "full"
+        w = 4 * nk + (1 if full else 0)
+        owner = ids // self.pu.block
+        counts = np.bincount(owner, minlength=world)
+        m = int(counts.max()) if n else 0
+        rows = torch.empty(n, w, dtype=torch.float64, device=dev)
+        if n:
+            k = int(counts[self.rank_id])
+            part = torch.zeros(m, w, dtype=torch.float64, device=dev)
+            part[:k, :4 * nk] = local["per_user"].reshape(k, 4 * nk)
+            if full:
+                part[:k, 4 * nk] = local["auc"]
+            if world > 1:
+                every = torch.empty(world * m, w, dtype=torch.float64, device=dev)
+                dist.all_gather_into_tensor(every, part, group=self.group)
+            else:
+                every = part
+            # owners in list order, grouped by rank: the r-th group is rank r's rows 0 .. counts[r] - 1
+            dst = np.argsort(owner, kind="stable")
+            src = np.concatenate([r * m + np.arange(counts[r], dtype=np.int64) for r in range(world)])
+            rows[torch.from_numpy(dst).to(dev)] = every[torch.from_numpy(src).to(dev)]
+        per_user = rows[:, :4 * nk].contiguous().view(n, 4, nk)
+        result = torch.zeros(4, nk, dtype=torch.float64, device=dev)
+        _lib.check(_lib.load().mmssl_eval_reduce(ptr(per_user), n, 4 * nk, ptr(result), stream()))
+        out = dict(per_user=per_user, result=result)
+        if full:
+            out["auc"] = rows[:, 4 * nk].contiguous()
+        return out
+
+    def rank(self, u_local: torch.Tensor, i_local: torch.Tensor, users_to_test, is_val: bool) -> Dict[str, torch.Tensor]:
+        """Collective.  Device tensors: result [4, nK] and per_user [n, 4, nK] fp64 in list order, in full mode auc [n] fp64; the
+        rank's own ranked / ranked_scores / hits rows and ``positions`` (host int64) -- where they stand in users_to_test."""
+        ids = self.check_users(users_to_test)
+        items = self.gather_items(i_local)
+        local, mine = self.rank_local(u_local, items, ids, is_val)
+        out = self.combine(local, ids)
+        out.update(ranked=local["ranked"], ranked_scores=local["ranked_scores"], hits=local["hits"], positions=torch.from_numpy(mine))
+        return out
+
+    def test_torch(self, u_local, i_local, users_to_test, is_val, drop_flag=False, batch_test_flag=False):
+        """Collective.  ``Evaluator.test_torch``'s result dict, identical on every rank."""
+        return _test_result(self.rank(u_local, i_local, users_to_test, is_val), self.test_flag, self.device)

@@ -450,6 +450,33 @@ class RowShardedHotStep:
                       self.step_dev, cfg.lr, cfg.beta1, cfg.beta2, cfg.eps, cfg.weight_decay)
         return self.out5
 
+    # -------------------------------------------------------------- evaluation
+    def _quiesce(self) -> None:
+        """With the multicast exchange a rank publishes into the symmetric tables of EVERY rank, and the captured step uses the
+        same tables: wait until no rank is inside a step or an exchange."""
+        if self.mc is not None:
+            torch.cuda.synchronize(self.idx.device)
+            dist.barrier(group=self.group)
+
+    def final_embeddings(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Collective.  The model's eval-mode forward (no dropout, no losses, no optimiser step) through the step's own exchange:
+        the rank's padded [block, d] rows of the final user and item tables (u_f, i_f), fresh tensors.  Writes nothing a later
+        step or a captured step reads: the forward allocates its outputs, and what it shares with the step -- the SpMM split-row
+        partials and the multicast exchange tables -- is scratch that every step writes before it reads (the barriers around
+        keep the ranks out of each other's exchanges).  The exchange counters keep counting training steps only."""
+        counters = (self.n_gathers, self.gathered_bytes, self.n_reduce_scatters)
+        self._quiesce()
+        outs, _ = self.engine.forward(self.P, self.feats, self.graphs, None, want_sumsq=False)
+        self._quiesce()
+        self.n_gathers, self.gathered_bytes, self.n_reduce_scatters = counters
+        return outs[0], outs[1]
+
+    def test(self, evaluator, users_to_test, is_val: bool) -> Dict[str, object]:
+        """Collective.  ``Trainer.test`` of the row-sharded model: ``evaluator`` is this rank's ``evaluate.ShardedEvaluator``;
+        returns its ``test_torch`` result, identical on every rank."""
+        u_f, i_f = self.final_embeddings()
+        return evaluator.test_torch(u_f, i_f, users_to_test, is_val)
+
     # -------------------------------------------------------------- checkpoint (checkpoint.py)
     def meta(self) -> dict:
         """Same fields as HotStep.meta; the training-matrix fingerprint is summed over the ranks' row blocks (a collective on the
