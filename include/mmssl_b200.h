@@ -296,6 +296,20 @@ int mmssl_sample_triples_multi(const int64_t* indptr, const int64_t* indices, co
                                int64_t n_items, int batch, uint64_t seed, const int32_t* step_dev, int32_t step_host,
                                void* workspace, int64_t workspace_bytes, int64_t* users, int64_t* pos, int64_t* neg,
                                void* stream);
+/* Row-sharded form of both paths: a rank holds the training rows of one block of users (indptr rebased to 0, int32 GLOBAL item
+ * ids, rows sorted); exist[] lists the block's non-empty local rows in ascending order, and they are the slots
+ * [slot_lo, slot_hi) of the GLOBAL order of non-empty rows (n_exist over all ranks); row0 is the block's first global user id.
+ * Every rank runs the same selection over n_exist (claim[n_exist] / the workspace are sized for it); an entry whose slot the
+ * rank owns holds the one-GPU sampler's triple (global ids), every other entry is 0.  Summing the ranks' outputs gives
+ * exactly the batch mmssl_sample_triples / mmssl_sample_triples_multi draw on the whole matrix. */
+int mmssl_sample_triples_owned(const int64_t* indptr, const int32_t* indices, const int64_t* exist, int64_t slot_lo,
+                               int64_t slot_hi, int64_t row0, int64_t n_exist, int64_t n_items, int batch, uint64_t seed,
+                               const int32_t* step_dev, int32_t step_host, int32_t* claim, int64_t* users, int64_t* pos,
+                               int64_t* neg, void* stream);
+int mmssl_sample_triples_multi_owned(const int64_t* indptr, const int32_t* indices, const int64_t* exist, int64_t slot_lo,
+                                     int64_t slot_hi, int64_t row0, int64_t n_exist, int64_t n_items, int batch, uint64_t seed,
+                                     const int32_t* step_dev, int32_t step_host, void* workspace, int64_t workspace_bytes,
+                                     int64_t* users, int64_t* pos, int64_t* neg, void* stream);
 
 /* ------------------------------------------------------------------ evaluation (SURVEY 8f "next" #3)
  * Trainer.test -> test_torch / test_one_user (main.py:301-306, utility/batch_test.py:21-36, :83-169) and
@@ -413,6 +427,12 @@ int mmssl_publish_rows(const float* src, int64_t lds, int64_t rows, int d, float
 /* All-reduce(sum) without NCCL: dst[0..n) = sum over the ranks' copies of a symmetric buffer, read through its multicast address
  * (multimem.ld_reduce, the switch adds the replicas).  The caller barriers all ranks before (contributions written) and after. */
 int mmssl_mc_allreduce_sum(const float* src_mc, float* dst, int64_t n, void* stream);
+/* The same, exact, for n 64-bit integers (ids that an fp32 sum would round): mmssl_ids_to_limbs writes a rank's ids into its copy
+ * of a symmetric fp32 buffer as four 16-bit limbs per id (dst[4n] floats); after the barrier mmssl_mc_allreduce_ids reads the
+ * limb sums through the buffer's multicast address (multimem.ld_reduce.add.v4.f32, exact below 2^24, i.e. for up to 256 ranks)
+ * and reassembles dst[i] = the integer sum of the ranks' ids mod 2^64. */
+int mmssl_ids_to_limbs(const int64_t* src, float* dst, int64_t n, void* stream);
+int mmssl_mc_allreduce_ids(const float* src_mc, int64_t* dst, int64_t n, void* stream);
 
 /* ------------------------------------------------------------------ modality-graph bookkeeping of the full step (regraph.cu)
  * mmssl_topk_rows: ids[rows, k] (int64) = columns of the k largest entries of every row of x[rows, w], best first, equal

@@ -110,6 +110,10 @@ _SIGS = {
     "mmssl_sampler_workspace_bytes": (c_i64, [c_i64, c_i32]),
     "mmssl_sample_triples_multi": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i32, C.c_uint64, c_vp, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp,
                                              c_vp]),
+    "mmssl_sample_triples_owned": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, C.c_uint64, c_vp, c_i32, c_vp,
+                                             c_vp, c_vp, c_vp, c_vp]),
+    "mmssl_sample_triples_multi_owned": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, C.c_uint64, c_vp, c_i32,
+                                                   c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]),
     "mmssl_eval_rank": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, C.POINTER(c_i32), c_i32,
                                   c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "mmssl_eval_full_stage": (C.c_int, []),
@@ -139,6 +143,8 @@ _SIGS = {
     "mmssl_scatter_add_owned": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, c_i32, c_vp, c_i64, c_vp]),
     "mmssl_publish_rows": (C.c_int, [c_vp, c_i64, c_i64, c_i32, c_vp, c_i64, c_i32, c_i32, C.POINTER(c_vp), c_vp]),
     "mmssl_mc_allreduce_sum": (C.c_int, [c_vp, c_vp, c_i64, c_vp]),
+    "mmssl_ids_to_limbs": (C.c_int, [c_vp, c_vp, c_i64, c_vp]),
+    "mmssl_mc_allreduce_ids": (C.c_int, [c_vp, c_vp, c_i64, c_vp]),
     "mmssl_topk_rows": (C.c_int, [c_vp, c_i64, c_i64, c_i64, c_i32, c_vp, c_vp]),
     "mmssl_pair_append": (C.c_int, [c_vp, c_i64, c_vp, c_i32, c_vp, c_vp, c_vp]),
     "mmssl_degree_values": (C.c_int, [c_vp, c_i64, c_i64, c_vp, c_vp, c_vp]),
@@ -169,14 +175,14 @@ KERNELS_PER_CALL = {
     "mmssl_dwcat_reduce": 1, "mmssl_combine_fwd": 1, "mmssl_combine_bwd": 1, "mmssl_softmax_bwd": 1,
     "mmssl_axpby": 1, "mmssl_mul_mask": 1, "mmssl_sumsq": 1, "mmssl_bpr": 1, "mmssl_infonce_prepare": 1,
     "mmssl_infonce_stats": 2, "mmssl_infonce_grad": 1, "mmssl_infonce_scatter": 1, "mmssl_infonce_stats_tc": 4, "mmssl_infonce_forward_tc": 3, "mmssl_infonce_grad_tc": 1, "mmssl_loss_assemble": 1,
-    "mmssl_step_tick": 1, "mmssl_dp_fused_adamw": 1, "mmssl_dp_fused_adamw_dev": 1, "mmssl_sampler_init": 1, "mmssl_sample_triples": 1, "mmssl_sample_triples_multi": 20, "mmssl_adamw": 1, "mmssl_split_bf16": 1, "mmssl_split_bf16_t": 1, "mmssl_split_bf16_t_colsum": 1, "mmssl_gemm_bf16x3": 1, "mmssl_gemm_bf16x3_group": 1, "mmssl_gemm_bf16x3_wide": 1,
+    "mmssl_step_tick": 1, "mmssl_dp_fused_adamw": 1, "mmssl_dp_fused_adamw_dev": 1, "mmssl_sampler_init": 1, "mmssl_sample_triples": 1, "mmssl_sample_triples_multi": 20, "mmssl_sample_triples_owned": 1, "mmssl_sample_triples_multi_owned": 20, "mmssl_adamw": 1, "mmssl_split_bf16": 1, "mmssl_split_bf16_t": 1, "mmssl_split_bf16_t_colsum": 1, "mmssl_gemm_bf16x3": 1, "mmssl_gemm_bf16x3_group": 1, "mmssl_gemm_bf16x3_wide": 1,
     "mmssl_proj_epilogue": 1, "mmssl_wgrad_epilogue": 1, "mmssl_colsum": 1,
     "mmssl_eval_rank": 1, "mmssl_eval_rank_full": 1, "mmssl_eval_rank_wide": 1, "mmssl_eval_reduce": 1,
     "mmssl_gan_bn_fwd": 1, "mmssl_gan_bn_bwd": 1, "mmssl_gan_gp_rev_bn": 1, "mmssl_gan_bn_fwd_rev": 1, "mmssl_gan_colsum": 1,
     "mmssl_gan_head_fwd": 2, "mmssl_gan_head_bwd": 1, "mmssl_gan_gp_rows": 2, "mmssl_gan_gp_head_rev": 2, "mmssl_gan_usim_finish": 1,
     "mmssl_gan_usim_bwd_pre": 1, "mmssl_gan_real_rows": 1, "mmssl_gan_interpolate": 1, "mmssl_gan_add_scaled": 1,
     "mmssl_gan_gather_rows": 1, "mmssl_gan_scatter_add_rows": 1,
-    "mmssl_topk_rows": 1, "mmssl_pair_append": 1, "mmssl_degree_values": 2, "mmssl_gather_owned": 1, "mmssl_scatter_add_owned": 1, "mmssl_publish_rows": 1, "mmssl_mc_allreduce_sum": 1,
+    "mmssl_topk_rows": 1, "mmssl_pair_append": 1, "mmssl_degree_values": 2, "mmssl_gather_owned": 1, "mmssl_scatter_add_owned": 1, "mmssl_publish_rows": 1, "mmssl_mc_allreduce_sum": 1, "mmssl_ids_to_limbs": 1, "mmssl_mc_allreduce_ids": 1,
 }
 launch_count = 0
 call_log = None   # set to a list to record (name) of every kernel-launching call

@@ -11,6 +11,8 @@
 // (seed, step), never on scheduling; the claim table cleans itself up.  Counter-based RNG
 // (splitmix64 of (seed, step, thread, draw)), so the kernel is replayable inside a CUDA graph with
 // the step number read from device memory.
+// Row-sharded runs (ShardedTripleSampler): the same kernels with an owned slot range -- every rank selects the slots over the
+// global n_exist, draws the triples of the slots whose users it holds and writes zeros elsewhere (draw_or_zero).
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -32,14 +34,18 @@ __device__ __forceinline__ uint32_t rnd32(uint64_t seed, uint32_t step, uint32_t
 // unbiased enough for sampling: 32-bit multiply-shift range reduction
 __device__ __forceinline__ uint32_t below(uint32_t r, uint32_t n) { return (uint32_t)(((uint64_t)r * n) >> 32); }
 
-// Triple t of the batch for the user exist[slot]: one uniform positive from the user's row, one uniform negative rejected
-// while it is in the row; `draw` is the next unused draw number of thread t.  Shared by both sampler paths.
-__device__ __forceinline__ void draw_triple(const int64_t* __restrict__ indptr, const int64_t* __restrict__ indices,
-                                            const int64_t* __restrict__ exist, int64_t slot, int64_t n_items, uint64_t seed,
-                                            uint32_t step, uint32_t t, uint32_t draw, int64_t* __restrict__ users,
-                                            int64_t* __restrict__ pos, int64_t* __restrict__ neg) {
-    const int64_t u = exist[slot];
-    const int64_t b = indptr[u], e = indptr[u + 1];
+// Triple t of the batch for the user of `slot`: one uniform positive from the user's row, one uniform negative rejected while it
+// is in the row; `draw` is the next unused draw number of thread t.  Shared by both sampler paths.
+// The rows are those of one block of users: the user of slot s is row0 + exist[s - slot_lo], whose row is indptr / indices of
+// that local row (indices: GLOBAL item ids, int64 on one GPU, int32 in a row block).  The one-GPU sampler passes the whole
+// matrix: slot_lo = row0 = 0.
+template <typename IdxT>
+__device__ __forceinline__ void draw_triple(const int64_t* __restrict__ indptr, const IdxT* __restrict__ indices,
+                                            const int64_t* __restrict__ exist, int64_t slot, int64_t slot_lo, int64_t row0,
+                                            int64_t n_items, uint64_t seed, uint32_t step, uint32_t t, uint32_t draw,
+                                            int64_t* __restrict__ users, int64_t* __restrict__ pos, int64_t* __restrict__ neg) {
+    const int64_t r = exist[slot - slot_lo];
+    const int64_t b = indptr[r], e = indptr[r + 1];
     const uint32_t deg = (uint32_t)(e - b);
     const int64_t p = indices[b + below(rnd32(seed, step, t, draw++), deg)];
     int64_t ng = 0;
@@ -48,17 +54,31 @@ __device__ __forceinline__ void draw_triple(const int64_t* __restrict__ indptr, 
         int64_t lo = b, hi = e;             // binary search in the (sorted) row
         while (lo < hi) {
             const int64_t mid = (lo + hi) >> 1;
-            if (indices[mid] < ng) lo = mid + 1; else hi = mid;
+            if ((int64_t)indices[mid] < ng) lo = mid + 1; else hi = mid;
         }
-        if (!(lo < e && indices[lo] == ng)) break;
+        if (!(lo < e && (int64_t)indices[lo] == ng)) break;
     }
-    users[t] = u; pos[t] = p; neg[t] = ng;
+    users[t] = row0 + r; pos[t] = p; neg[t] = ng;
 }
 
+// Row-sharded form (kOwned): every rank runs the same slot selection over the GLOBAL n_exist, and thread t draws its triple only
+// when its slot lies in the rank's range [slot_lo, slot_hi); every other entry is written as zero, so each entry of the batch has
+// exactly one writer over the ranks and an integer sum over the ranks is the one-GPU batch.
+template <typename IdxT, bool kOwned>
+__device__ __forceinline__ void draw_or_zero(const int64_t* __restrict__ indptr, const IdxT* __restrict__ indices,
+                                             const int64_t* __restrict__ exist, int64_t slot, int64_t slot_lo, int64_t slot_hi,
+                                             int64_t row0, int64_t n_items, uint64_t seed, uint32_t step, uint32_t t, uint32_t draw,
+                                             int64_t* __restrict__ users, int64_t* __restrict__ pos, int64_t* __restrict__ neg) {
+    if (kOwned && (slot < slot_lo || slot >= slot_hi)) { users[t] = 0; pos[t] = 0; neg[t] = 0; return; }
+    // the one-GPU instances see constant zeros: no new work in them
+    draw_triple(indptr, indices, exist, slot, kOwned ? slot_lo : 0, kOwned ? row0 : 0, n_items, seed, step, t, draw, users, pos, neg);
+}
+
+template <typename IdxT, bool kOwned>
 __global__ void __launch_bounds__(1024) sample_triples_kernel(const int64_t* __restrict__ indptr,
-                                                              const int64_t* __restrict__ indices,
-                                                              const int64_t* __restrict__ exist, int64_t n_exist,
-                                                              int64_t n_items, int batch, uint64_t seed,
+                                                              const IdxT* __restrict__ indices,
+                                                              const int64_t* __restrict__ exist, int64_t slot_lo, int64_t slot_hi,
+                                                              int64_t row0, int64_t n_exist, int64_t n_items, int batch, uint64_t seed,
                                                               const int32_t* __restrict__ step_dev, int32_t step_host,
                                                               int32_t* __restrict__ claim, int64_t* __restrict__ users,
                                                               int64_t* __restrict__ pos, int64_t* __restrict__ neg) {
@@ -95,7 +115,7 @@ __global__ void __launch_bounds__(1024) sample_triples_kernel(const int64_t* __r
     if (t < batch && !with_replacement && slot >= 0) claim[slot] = 0x7fffffff;   // leave the table clean
     if (t >= batch) return;
     if (slot < 0) slot = below(rnd32(seed, step, t, draw++), (uint32_t)n_exist);  // (never in practice: 64 rounds)
-    draw_triple(indptr, indices, exist, slot, n_items, seed, step, t, draw, users, pos, neg);
+    draw_or_zero<IdxT, kOwned>(indptr, indices, exist, slot, slot_lo, slot_hi, row0, n_items, seed, step, t, draw, users, pos, neg);
 }
 
 __global__ void fill_claim_kernel(int32_t* claim, int64_t n) {
@@ -203,8 +223,10 @@ __global__ void __launch_bounds__(kSelThreads) select_compact_kernel(uint64_t se
 }
 
 // Triple t: the user of sorted slot t, or (batch > n_exist) a uniform slot with replacement, as in sample_triples_kernel
-__global__ void __launch_bounds__(256) sample_draw_kernel(const int64_t* __restrict__ indptr, const int64_t* __restrict__ indices,
-                                                          const int64_t* __restrict__ exist, int64_t n_exist, int64_t n_items, int batch,
+template <typename IdxT, bool kOwned>
+__global__ void __launch_bounds__(256) sample_draw_kernel(const int64_t* __restrict__ indptr, const IdxT* __restrict__ indices,
+                                                          const int64_t* __restrict__ exist, int64_t slot_lo, int64_t slot_hi,
+                                                          int64_t row0, int64_t n_exist, int64_t n_items, int batch,
                                                           uint64_t seed, const int32_t* __restrict__ step_dev, int32_t step_host,
                                                           const int32_t* __restrict__ slots, int64_t* __restrict__ users,
                                                           int64_t* __restrict__ pos, int64_t* __restrict__ neg) {
@@ -213,7 +235,8 @@ __global__ void __launch_bounds__(256) sample_draw_kernel(const int64_t* __restr
     const uint32_t step = (uint32_t)(step_dev ? *step_dev : step_host);
     uint32_t draw = 0;
     const int64_t slot = slots ? (int64_t)slots[t] : (int64_t)below(rnd32(seed, step, (uint32_t)t, draw++), (uint32_t)n_exist);
-    draw_triple(indptr, indices, exist, slot, n_items, seed, step, (uint32_t)t, draw, users, pos, neg);
+    draw_or_zero<IdxT, kOwned>(indptr, indices, exist, slot, slot_lo, slot_hi, row0, n_items, seed, step, (uint32_t)t, draw, users, pos,
+                               neg);
 }
 
 struct SelectWs {
@@ -243,40 +266,23 @@ static cudaError_t select_carve(int64_t batch, int64_t n_exist, void* base, Sele
     return cudaSuccess;
 }
 
-}  // namespace mmssl
-
-using namespace mmssl;
-
-extern "C" int mmssl_sampler_init(int32_t* claim, int64_t n_exist, void* stream_) {
-    if (n_exist == 0) return 0;
-    fill_claim_kernel<<<(unsigned)((n_exist + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(claim, n_exist);
-    MMSSL_LAUNCH_OK();
-    return 0;
-}
-
-extern "C" int mmssl_sample_triples(const int64_t* indptr, const int64_t* indices, const int64_t* exist, int64_t n_exist,
-                                    int64_t n_items, int batch, uint64_t seed, const int32_t* step_dev, int32_t step_host,
-                                    int32_t* claim, int64_t* users, int64_t* pos, int64_t* neg, void* stream_) {
+// The two sampler paths for one index type and ownership; the extern "C" entry points below only pick the instance.
+template <typename IdxT, bool kOwned>
+static int sample_one_cta(const int64_t* indptr, const IdxT* indices, const int64_t* exist, int64_t slot_lo, int64_t slot_hi, int64_t row0,
+                          int64_t n_exist, int64_t n_items, int batch, uint64_t seed, const int32_t* step_dev, int32_t step_host,
+                          int32_t* claim, int64_t* users, int64_t* pos, int64_t* neg, cudaStream_t st) {
     MMSSL_REQUIRE(batch >= 1 && batch <= 1024, "one sampler launch draws at most 1024 triples (larger batches: mmssl_sample_triples_multi)");
     MMSSL_REQUIRE(n_exist >= 1 && n_exist < (1ll << 31) && n_items >= 1 && n_items < (1ll << 31), "bad sizes");
-    sample_triples_kernel<<<1, 1024, 0, (cudaStream_t)stream_>>>(indptr, indices, exist, n_exist, n_items, batch, seed, step_dev,
-                                                                  step_host, claim, users, pos, neg);
+    sample_triples_kernel<IdxT, kOwned><<<1, 1024, 0, st>>>(indptr, indices, exist, slot_lo, slot_hi, row0, n_exist, n_items, batch, seed,
+                                                            step_dev, step_host, claim, users, pos, neg);
     MMSSL_LAUNCH_OK();
     return 0;
 }
 
-extern "C" int64_t mmssl_sampler_workspace_bytes(int64_t n_exist, int batch) {
-    if (batch < 1 || batch > n_exist) return 0;     // with replacement: no selection
-    SelectWs w;
-    if (select_carve(batch, n_exist, nullptr, &w) != cudaSuccess) return -1;
-    return (int64_t)w.total;
-}
-
-extern "C" int mmssl_sample_triples_multi(const int64_t* indptr, const int64_t* indices, const int64_t* exist, int64_t n_exist,
-                                          int64_t n_items, int batch, uint64_t seed, const int32_t* step_dev, int32_t step_host,
-                                          void* workspace, int64_t workspace_bytes, int64_t* users, int64_t* pos, int64_t* neg,
-                                          void* stream_) {
-    cudaStream_t st = (cudaStream_t)stream_;
+template <typename IdxT, bool kOwned>
+static int sample_multi(const int64_t* indptr, const IdxT* indices, const int64_t* exist, int64_t slot_lo, int64_t slot_hi, int64_t row0,
+                        int64_t n_exist, int64_t n_items, int batch, uint64_t seed, const int32_t* step_dev, int32_t step_host,
+                        void* workspace, int64_t workspace_bytes, int64_t* users, int64_t* pos, int64_t* neg, cudaStream_t st) {
     MMSSL_REQUIRE(batch >= 1, "batch must be positive");
     MMSSL_REQUIRE(n_exist >= 1 && n_exist < (1ll << 31) && n_items >= 1 && n_items < (1ll << 31), "bad sizes");
     const int32_t* slots = nullptr;
@@ -295,8 +301,66 @@ extern "C" int mmssl_sample_triples_multi(const int64_t* indptr, const int64_t* 
         MMSSL_CUDA(cub::DeviceRadixSort::SortPairs(w.cub_tmp, cub_bytes, w.keys_in, w.keys_out, w.slots_in, w.slots_out, batch, 0, 32 + slot_bits(n_exist), st));
         slots = w.slots_out;
     }
-    sample_draw_kernel<<<(unsigned)((batch + 255) / 256), 256, 0, st>>>(indptr, indices, exist, n_exist, n_items, batch, seed, step_dev,
-                                                                         step_host, slots, users, pos, neg);
+    sample_draw_kernel<IdxT, kOwned><<<(unsigned)((batch + 255) / 256), 256, 0, st>>>(indptr, indices, exist, slot_lo, slot_hi, row0, n_exist,
+                                                                                      n_items, batch, seed, step_dev, step_host, slots, users,
+                                                                                      pos, neg);
     MMSSL_LAUNCH_OK();
     return 0;
+}
+
+// The owned slot range of a rank: [slot_lo, slot_hi) inside [0, n_exist), exist[] holds slot_hi - slot_lo local rows.
+static int check_owned(int64_t slot_lo, int64_t slot_hi, int64_t row0, int64_t n_exist) {
+    MMSSL_REQUIRE(slot_lo >= 0 && slot_lo <= slot_hi && slot_hi <= n_exist && row0 >= 0, "owned slot range outside [0, n_exist)");
+    return 0;
+}
+
+}  // namespace mmssl
+
+using namespace mmssl;
+
+extern "C" int mmssl_sampler_init(int32_t* claim, int64_t n_exist, void* stream_) {
+    if (n_exist == 0) return 0;
+    fill_claim_kernel<<<(unsigned)((n_exist + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(claim, n_exist);
+    MMSSL_LAUNCH_OK();
+    return 0;
+}
+
+extern "C" int mmssl_sample_triples(const int64_t* indptr, const int64_t* indices, const int64_t* exist, int64_t n_exist,
+                                    int64_t n_items, int batch, uint64_t seed, const int32_t* step_dev, int32_t step_host,
+                                    int32_t* claim, int64_t* users, int64_t* pos, int64_t* neg, void* stream_) {
+    return sample_one_cta<int64_t, false>(indptr, indices, exist, 0, n_exist, 0, n_exist, n_items, batch, seed, step_dev, step_host, claim,
+                                          users, pos, neg, (cudaStream_t)stream_);
+}
+
+extern "C" int64_t mmssl_sampler_workspace_bytes(int64_t n_exist, int batch) {
+    if (batch < 1 || batch > n_exist) return 0;     // with replacement: no selection
+    SelectWs w;
+    if (select_carve(batch, n_exist, nullptr, &w) != cudaSuccess) return -1;
+    return (int64_t)w.total;
+}
+
+extern "C" int mmssl_sample_triples_multi(const int64_t* indptr, const int64_t* indices, const int64_t* exist, int64_t n_exist,
+                                          int64_t n_items, int batch, uint64_t seed, const int32_t* step_dev, int32_t step_host,
+                                          void* workspace, int64_t workspace_bytes, int64_t* users, int64_t* pos, int64_t* neg,
+                                          void* stream_) {
+    return sample_multi<int64_t, false>(indptr, indices, exist, 0, n_exist, 0, n_exist, n_items, batch, seed, step_dev, step_host, workspace,
+                                        workspace_bytes, users, pos, neg, (cudaStream_t)stream_);
+}
+
+extern "C" int mmssl_sample_triples_owned(const int64_t* indptr, const int32_t* indices, const int64_t* exist, int64_t slot_lo,
+                                          int64_t slot_hi, int64_t row0, int64_t n_exist, int64_t n_items, int batch, uint64_t seed,
+                                          const int32_t* step_dev, int32_t step_host, int32_t* claim, int64_t* users, int64_t* pos,
+                                          int64_t* neg, void* stream_) {
+    if (int rc = check_owned(slot_lo, slot_hi, row0, n_exist)) return rc;
+    return sample_one_cta<int32_t, true>(indptr, indices, exist, slot_lo, slot_hi, row0, n_exist, n_items, batch, seed, step_dev, step_host,
+                                         claim, users, pos, neg, (cudaStream_t)stream_);
+}
+
+extern "C" int mmssl_sample_triples_multi_owned(const int64_t* indptr, const int32_t* indices, const int64_t* exist, int64_t slot_lo,
+                                                int64_t slot_hi, int64_t row0, int64_t n_exist, int64_t n_items, int batch, uint64_t seed,
+                                                const int32_t* step_dev, int32_t step_host, void* workspace, int64_t workspace_bytes,
+                                                int64_t* users, int64_t* pos, int64_t* neg, void* stream_) {
+    if (int rc = check_owned(slot_lo, slot_hi, row0, n_exist)) return rc;
+    return sample_multi<int32_t, true>(indptr, indices, exist, slot_lo, slot_hi, row0, n_exist, n_items, batch, seed, step_dev, step_host,
+                                       workspace, workspace_bytes, users, pos, neg, (cudaStream_t)stream_);
 }

@@ -122,6 +122,51 @@ extern "C" int mmssl_mc_allreduce_sum(const float* src_mc, float* dst, int64_t n
     return 0;
 }
 
+// ---- exact all-reduce(sum) of 64-bit integers (the row-sharded sampler's batch ids) through the same fp32 multicast reduction:
+// an fp32 sum of the ids themselves would round them above 2^24, so each id travels as four 16-bit limbs held as floats
+// (ids_to_limbs_kernel writes a rank's contribution into its copy of the symmetric buffer, one float4 per id).
+// multimem.ld_reduce.add.v4.f32 then adds each limb over the ranks; a limb sum is an integer below 256 * 2^16 < 2^24 for up to
+// 256 ranks, so fp32 holds it exactly, and the reassembled value is the exact integer sum mod 2^64.  The row-sharded sampler has
+// one writer per entry (zeros elsewhere): the sum is that writer's id.
+namespace mmssl {
+__global__ void __launch_bounds__(256) ids_to_limbs_kernel(const uint64_t* __restrict__ src, float* __restrict__ dst, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) {
+        const uint64_t v = src[i];
+        st4(dst + i * 4, make_float4((float)(v & 0xFFFFu), (float)((v >> 16) & 0xFFFFu), (float)((v >> 32) & 0xFFFFu), (float)(v >> 48)));
+    }
+}
+
+__global__ void __launch_bounds__(256) mc_allreduce_ids_kernel(const float* src_mc, uint64_t* __restrict__ dst, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) {
+        float4 v;
+        asm volatile("multimem.ld_reduce.relaxed.sys.global.add.v4.f32 {%0, %1, %2, %3}, [%4];"
+                     : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(src_mc + i * 4) : "memory");
+        dst[i] = (uint64_t)v.x + ((uint64_t)v.y << 16) + ((uint64_t)v.z << 32) + ((uint64_t)v.w << 48);
+    }
+}
+
+static unsigned id_blocks(int64_t n) {
+    const int64_t b = (n + 255) / 256;
+    return (unsigned)(b > kNumSMs * 8 ? kNumSMs * 8 : b);
+}
+}  // namespace mmssl
+
+extern "C" int mmssl_ids_to_limbs(const int64_t* src, float* dst, int64_t n, void* stream_) {
+    MMSSL_REQUIRE(n >= 0 && ((uintptr_t)src % 8) == 0 && aligned16(dst), "8-byte aligned ids, 16-byte aligned limb buffer");
+    if (n == 0) return 0;
+    ids_to_limbs_kernel<<<id_blocks(n), 256, 0, (cudaStream_t)stream_>>>(reinterpret_cast<const uint64_t*>(src), dst, n);
+    MMSSL_LAUNCH_OK();
+    return 0;
+}
+
+extern "C" int mmssl_mc_allreduce_ids(const float* src_mc, int64_t* dst, int64_t n, void* stream_) {
+    MMSSL_REQUIRE(n >= 0 && aligned16(src_mc) && ((uintptr_t)dst % 8) == 0, "16-byte aligned limb buffer, 8-byte aligned ids");
+    if (n == 0) return 0;
+    mc_allreduce_ids_kernel<<<id_blocks(n), 256, 0, (cudaStream_t)stream_>>>(src_mc, reinterpret_cast<uint64_t*>(dst), n);
+    MMSSL_LAUNCH_OK();
+    return 0;
+}
+
 // ---- reduce-scatter + SpMM epilogue of the row-sharded step's "partial product" schedule (rowshard_step.py): for a product
 // whose dense operand lives in the LARGE (user) row space, every rank multiplies the column block of A it owns,
 // A[:, U_r] * X[U_r], into its copy of a full-height partial table (symmetric memory).  After a barrier this kernel gives a rank

@@ -156,11 +156,14 @@ class MulticastExchange:
 class MulticastAllReduce:
     """Sum over the ranks of a flat fp32 buffer without NCCL: ``buffer`` (this rank's copy of a symmetric allocation) is where
     the contribution is written; ``reduce_into(out)`` = barrier, one kernel reading the sum through the multicast address
-    (mmssl_mc_allreduce_sum), barrier.  Needs an NVSwitch multicast address (raises otherwise: the caller keeps NCCL then)."""
+    (mmssl_mc_allreduce_sum), barrier.  Needs an NVSwitch multicast address (raises otherwise: the caller keeps NCCL then).
+    ``ids=True``: an exact sum of ``numel`` int64 values instead -- ``write_ids(src)`` stores the contribution as four 16-bit limbs
+    per value (mmssl_ids_to_limbs), ``reduce_into(out)`` reassembles the int64 sums (mmssl_mc_allreduce_ids)."""
 
-    def __init__(self, numel: int, device, group=None):
+    def __init__(self, numel: int, device, group=None, ids: bool = False):
         import torch.distributed._symmetric_memory as symm
-        n = (numel + 3) // 4 * 4
+        self.ids = ids
+        n = 4 * numel if ids else (numel + 3) // 4 * 4
         g = group if group is not None else dist.group.WORLD
         self.buffer = symm.empty(n, dtype=torch.float32, device=device)
         self.buffer.zero_()
@@ -171,12 +174,22 @@ class MulticastAllReduce:
         torch.cuda.synchronize(device)
         self.h.barrier()
 
+    def write_ids(self, src: torch.Tensor) -> None:
+        lib = _lib.load(require_device=True)
+        assert self.ids and src.dtype == torch.int64 and src.is_contiguous() and 4 * src.numel() <= self.buffer.numel()
+        _lib.check(lib.mmssl_ids_to_limbs(ptr(src), ptr(self.buffer), src.numel(), stream()))
+
     def reduce_into(self, out: torch.Tensor) -> torch.Tensor:
         import ctypes as C
         lib = _lib.load(require_device=True)
-        assert out.is_contiguous() and out.numel() % 4 == 0 and out.numel() <= self.buffer.numel()
+        assert out.is_contiguous()
         self.h.barrier()                         # every rank's contribution is in its copy
-        _lib.check(lib.mmssl_mc_allreduce_sum(C.c_void_p(self.mc), ptr(out), out.numel(), stream()))
+        if self.ids:
+            assert out.dtype == torch.int64 and 4 * out.numel() <= self.buffer.numel()
+            _lib.check(lib.mmssl_mc_allreduce_ids(C.c_void_p(self.mc), ptr(out), out.numel(), stream()))
+        else:
+            assert out.numel() % 4 == 0 and out.numel() <= self.buffer.numel()
+            _lib.check(lib.mmssl_mc_allreduce_sum(C.c_void_p(self.mc), ptr(out), out.numel(), stream()))
         self.h.barrier()                         # every rank has read: the buffer may be rewritten
         return out
 
@@ -242,8 +255,13 @@ class RowShardedHotStep:
 
     def __init__(self, params: Dict[str, torch.Tensor], feats: Sequence[FeatureStore], graphs: Sequence[RowBlockGraph],
                  cfg: HotStepConfig, batch: int, part_u: RowPartition, part_i: RowPartition, rank: int, group=None,
-                 optimizer_step: bool = True, exchange: str = "nccl", schedule: str = "reduce_scatter"):
+                 optimizer_step: bool = True, exchange: str = "nccl", schedule: str = "reduce_scatter", sampler=None):
         self.cfg, self.batch, self.pu, self.pi, self.rank, self.group = cfg, batch, part_u, part_i, rank, group
+        # optional sampler.ShardedTripleSampler: every run() draws the batch of (seed, step_dev) on the device, so every replay of
+        # a captured step trains on a fresh batch; without it the batch is what set_indices wrote
+        self.sampler = sampler
+        if sampler is not None:
+            sampler.reserve(batch)
         self.P = {k: params[k] for k in LIVE}
         self.feats, self.graphs = tuple(feats), tuple(graphs)
         self.engine = Engine(cfg.embed_size, cfg.n_layers, cfg.head_num, cfg.id_cat_rate, cfg.model_cat_rate, cfg.proj_impl)
@@ -383,7 +401,8 @@ class RowShardedHotStep:
 
     # -------------------------------------------------------------- one step
     def run(self) -> torch.Tensor:
-        """One hot step on the batch in ``self.idx`` (GLOBAL user / item ids, identical on every rank).  Returns the device
+        """One hot step on the batch in ``self.idx`` (GLOBAL user / item ids, identical on every rank; drawn into it first when
+        the step has a sampler).  Returns the device
         tensor [total, mf, emb, feat_reg, cl] -- global values, identical on every rank."""
         cfg, B = self.cfg, self.batch
         users, pos, neg = self.idx[0], self.idx[1], self.idx[2]
@@ -394,6 +413,8 @@ class RowShardedHotStep:
         outs, st = self.engine.forward(self.P, self.feats, self.graphs, self._masks(), want_sumsq=True)
         u_f, i_f, _, _, _, _, u_vid, u_tid, _, _ = outs
         alias = self.alias
+        if self.sampler is not None:                        # (seed, optimiser step) -> the batch, identical on every rank
+            self.sampler.sample_into(self.idx, step_dev=self.step_dev)
         # ---- the batch rows of the full tables: owned rows + one all-reduce
         part = self.rows_part
         gather_owned(u_f, users, ulo, uhi, part[0])
@@ -490,7 +511,10 @@ class RowShardedHotStep:
                 v = [int(x) for x in t.cpu()]
                 h, nnz = sum(v[j] << (16 * j) for j in range(4)) & ((1 << 64) - 1), v[4]
             self._fingerprint = (nnz, h)
-        return checkpoint.make_meta(self.pu.n, self.pi.n, self.cfg, self.batch, self.feats, self._fingerprint)
+        m = checkpoint.make_meta(self.pu.n, self.pi.n, self.cfg, self.batch, self.feats, self._fingerprint)
+        if self.sampler is not None:         # the batch of (seed, step) does not depend on the world size
+            m["sampler_seed"] = int(self.sampler.seed)
+        return m
 
     _fingerprint = None
 
@@ -527,13 +551,16 @@ class RowShardedHotStep:
 
     # -------------------------------------------------------------- CUDA graph
     def capture(self, warmup: int = 2) -> None:
-        """Capture ``run`` into a CUDA graph (static buffers; update the indices with ``set_indices`` between replays).  Only with the
+        """Capture ``run`` into a CUDA graph (static buffers; update the indices with ``set_indices`` between replays, or give the
+        step a sampler: each replay then draws the batch of its step).  Only with the
         multicast exchange or a single rank: every exchange is then a kernel plus a device-side signal-pad barrier, which a graph
         can hold; NCCL collectives inside a capture hung in round 1 and are refused here.  EXPERIMENTAL until its first GPU run."""
         if self.pu.world > 1 and self.mc is None:
             raise RuntimeError("capture() needs exchange='multicast' (NCCL collectives are not captured)")
         if self.pu.world > 1 and self.ar_rows is None:
             raise RuntimeError("capture() needs the multicast all-reduce (no NVSwitch multicast address on this system)")
+        if self.sampler is not None and self.sampler.exchange is not None and self.sampler.ar.get(self.batch) is None:
+            raise RuntimeError("capture() needs a sampler with exchange='multicast' (its NCCL all-reduce is not captured)")
 
         def warm():
             for _ in range(warmup):

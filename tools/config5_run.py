@@ -9,7 +9,10 @@ permutation, duplicate (u, i) pairs dropped (so the edge count ends slightly bel
 csr_norm(mean_flag=True) (main.py:89-103): (deg_row + 1e-8)^-1/2 on each side.  It keeps its row blocks (and the column blocks of
 the partial-product schedule), its rows of the features / tables, and runs RowShardedHotStep (multicast exchange, reduce-scatter
 schedule, CUDA graph).  Prints one JSON line (rank 0): ms/step, exchanges and bytes per step, peak memory per rank.
-No 1-GPU twin is built at this size: parity of the same code path is checked at Sports / 1M x 200k by bench.py --gpus N."""
+No 1-GPU twin is built at this size: parity of the same code path is checked at Sports / 1M x 200k by bench.py --gpus N.
+By default every step trains on one batch drawn once from the edge list.  With --sampler device each rank builds the training rows
+of its user block from the edges it keeps, and every step (every graph replay) draws a fresh batch of Data.sample on the device
+(sampler.ShardedTripleSampler: bitwise the one-GPU device sampler's batch at that step, at any world size)."""
 import argparse
 import json
 import os
@@ -33,6 +36,8 @@ ap.add_argument("--batch", type=int, default=1024)
 ap.add_argument("--steps", type=int, default=5)
 ap.add_argument("--seed", type=int, default=2022)
 ap.add_argument("--no-graph", action="store_true")
+ap.add_argument("--sampler", choices=("fixed", "device"), default="fixed",
+                help="fixed: one batch for every step; device: a fresh batch per step, drawn on the rank that holds the user's row")
 a = ap.parse_args()
 
 rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
@@ -105,6 +110,15 @@ bu = torch.randperm(U, generator=g, device=dev)[:a.batch]
 first = torch.searchsorted(rows, bu)
 pos = cols[first.clamp_(max=nnz - 1)]
 neg = torch.randint(0, I, (a.batch,), generator=g, device=dev)
+smp = None
+if a.sampler == "device":                               # the rank's training rows: its edges, sorted by (user, item) already
+    from mmssl_b200.dataset import CsrBlock  # noqa: E402
+    from mmssl_b200.sampler import ShardedTripleSampler  # noqa: E402
+    indptr = torch.zeros(pu.block + 1, dtype=torch.int64, device=dev)
+    indptr[1:] = torch.cumsum(torch.bincount(rows[mu] - ulo, minlength=pu.block), 0)
+    blk = CsrBlock(indptr.cpu().numpy(), cols[mu].to(torch.int32).cpu().numpy(), None, (pu.block, I), ulo, uhi)
+    smp = ShardedTripleSampler(blk, pu, rank, device=dev, seed=a.seed, exchange="multicast" if world > 1 else "nccl")
+    del indptr, blk
 del rows, cols, v_ui, v_iu, mu, mi
 torch.cuda.empty_cache()
 
@@ -126,8 +140,8 @@ gen_s = time.perf_counter() - t0
 
 cfg = HotStepConfig(embed_size=d, n_layers=a.layers, batch_size=a.batch)
 sh = RowShardedHotStep(P, feats, (g_ui, g_iu, g_ui, g_iu, g_ui, g_iu), cfg, a.batch, pu, pi, rank,
-                       exchange="multicast" if world > 1 else "nccl", schedule="reduce_scatter")
-sh.set_indices(bu, pos, neg)
+                       exchange="multicast" if world > 1 else "nccl", schedule="reduce_scatter", sampler=smp)
+sh.set_indices(bu, pos, neg)                             # (overwritten by every step when the sampler draws the batch)
 out = sh.run().clone()                                   # first eager step (creates the symmetric tables)
 torch.cuda.synchronize()
 captured = False
@@ -160,6 +174,7 @@ else:
     gath, rsc, gbytes = sh.n_gathers, sh.n_reduce_scatters, float(sh.gathered_bytes)
 if rank == 0:
     print(json.dumps({"workload": f"synthetic bipartite {U}x{I}, {nnz} edges (requested {a.edges}), d={d}, {a.layers}-layer GCN, V{a.dv}/T{a.dt}, global B={a.batch}",
+                      "batches": "device sampler, fresh per step" if smp is not None else "one fixed batch",
                       "n_gpus": world, "scheme": "row-sharded whole hot step (multicast exchange, reduce-scatter schedule)", "cuda_graph": captured,
                       "ms_per_step": round(float(ms), 3), "triples_per_s": round(a.batch / float(ms) * 1e3, 1), "loss_first_step": [round(float(x), 6) for x in out],
                       "all_gathers_per_step": int(gath), "reduce_scatters_per_step": int(rsc), "bytes_received_per_rank_per_step": int(gbytes),
