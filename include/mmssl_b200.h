@@ -356,6 +356,17 @@ int mmssl_eval_rank_wide(const float* user_emb, int64_t ldu, const float* item_e
                          double* auc_per_user, uint32_t* pos_ws, const int64_t* pos_ws_off, uint64_t* key_ws, void* stream);
 int mmssl_eval_reduce(const double* per_user, int64_t n_eval, int n_metrics, double* result, void* stream);
 
+/* Recommendation: the k best items of users[n] (best first, equal scores: lower item id first) among the items their row of
+ * the exclusion CSR (excl_indptr / excl_indices, int64, rows SORTED) does not name -- the ranking of mmssl_eval_rank (k <= 64)
+ * or mmssl_eval_rank_wide (k > 64) with Ks = [k] and the exclusion rows as training rows, so the lists are the evaluator's
+ * ranked / ranked_scores bit for bit; no held-out rows, hits or metrics.  ids[n, ldo] int32 (-1 past the end of a short list),
+ * scores[n, ldo] fp32 (0 there; may be NULL), ldo >= k, so a chunk of users writes into its rows of a larger buffer.  key_ws
+ * must hold mmssl_recommend_workspace_bytes(n, k, n_items, d) bytes (as mmssl_eval_rank_wide's; 0 for k <= 64). */
+int64_t mmssl_recommend_workspace_bytes(int64_t n, int k, int64_t n_items, int d);
+int mmssl_recommend_topk(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
+                         const int64_t* users, int64_t n, const int64_t* excl_indptr, const int64_t* excl_indices, int k,
+                         int64_t ldo, int32_t* ids, float* scores, uint64_t* key_ws, void* stream);
+
 /* ------------------------------------------------------------------ GAN side (SURVEY 8f "next" #2), see csrc/gan.cu
  * Device ops sequenced by mmssl_b200/gan.py; the Discriminator of Models.py:224-245 on n rows (LeakyReLU(True) is the
  * identity and does not appear), gradient_penalty main.py:140-160, u_sim_calculation main.py:283-298, the real rows of

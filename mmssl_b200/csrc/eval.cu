@@ -28,6 +28,10 @@
 // takes any list) runs on eval_wide_kernel: the same tile, sweep and AUC code (eval_sweep, eval_positives, eval_auc_finish),
 // buffers sized from max(Ks) in shared memory or a per-CTA workspace slot, an exact radix select as compaction, one radix
 // sort at the end and the metrics of any number of cut-offs in one walk over the ranked list.
+//
+// Recommendation (mmssl_recommend_topk) is the kRec instantiation of both kernels: the same tile, sweep, buffers, compaction
+// and keys against an exclusion CSR in place of the training rows, one k, no held-out rows, no hits and no metrics; the best k
+// of each user go to ids / scores rows of leading dimension ldo.
 #include "common.cuh"
 #include "../../include/mmssl_b200.h"
 
@@ -122,6 +126,22 @@ __device__ __forceinline__ void eval_dot(const float* __restrict__ row, const fl
     }
 #pragma unroll
     for (int u = 0; u < NU; ++u) s[u] = s[u] + 0.0f;
+}
+
+// Recommendation mode: the m <= kmax sorted keys of one user -> ids / scores[0, kmax) (-1 / 0 past m), one warp.
+__device__ __forceinline__ void eval_write_list(const uint64_t* sk, int m, int kmax, int32_t* __restrict__ ids,
+                                                float* __restrict__ scores, int lane) {
+    for (int pos = lane; pos < kmax; pos += 32) {
+        int32_t item = -1;
+        float sc = 0.f;
+        if (pos < m) {
+            const uint64_t key = sk[pos];
+            item = (int32_t)(0xFFFFFFFFu - (uint32_t)key);
+            sc = eval_key_score(key);
+        }
+        ids[pos] = item;
+        if (scores) scores[pos] = sc;
+    }
 }
 
 // ---- full mode (test_flag == 'full', batch_test.py:38-68): per-user ROC-AUC over all non-training items.
@@ -336,13 +356,16 @@ __device__ __forceinline__ void eval_auc_finish(EvalTile& t, unsigned long long 
     }
 }
 
-template <bool kFull>
+// kRec (recommendation): tr_* is the exclusion CSR, he_* / hits_out / per_user are unused, ks holds the one k, and ranked /
+// ranked_scores are rows of leading dimension ldo.
+template <bool kFull, bool kRec = false>
 __global__ void __launch_bounds__(kEvalThreads, kFull ? 2 : 0) eval_rank_kernel(
     const float* __restrict__ user_emb, int64_t ldu, const float* __restrict__ item_emb, int64_t ldi, int64_t n_items, int d,
     const int64_t* __restrict__ users, int64_t n_eval, const int64_t* __restrict__ tr_ptr, const int64_t* __restrict__ tr_idx,
     const int64_t* __restrict__ he_ptr, const int64_t* __restrict__ he_idx, EvalKs ks, int32_t* __restrict__ ranked,
     float* __restrict__ ranked_scores, int32_t* __restrict__ hits_out, double* __restrict__ per_user, float* __restrict__ scores_out,
-    double* __restrict__ auc_out, uint32_t* pos_ws, const int64_t* __restrict__ pos_ws_off) {
+    double* __restrict__ auc_out, uint32_t* pos_ws, const int64_t* __restrict__ pos_ws_off, int64_t ldo) {
+    static_assert(!(kFull && kRec), "recommendation has no full mode");
     extern __shared__ __align__(16) unsigned char eval_smem[];
     uint64_t (*keys)[kEvalCap] = reinterpret_cast<uint64_t (*)[kEvalCap]>(eval_smem);
     float* uvec = reinterpret_cast<float*>(eval_smem + sizeof(uint64_t) * kEvalUsers * kEvalCap);
@@ -352,7 +375,7 @@ __global__ void __launch_bounds__(kEvalThreads, kFull ? 2 : 0) eval_rank_kernel(
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int64_t tile0 = (int64_t)blockIdx.x * kEvalUsers;
-    if (tid < kEvalMaxK) disc[tid] = 1.0 / log2((double)(tid + 2));      // metrics.py:54
+    if (!kRec && tid < kEvalMaxK) disc[tid] = 1.0 / log2((double)(tid + 2));      // metrics.py:54
     eval_tile_begin<kFull>(t, uvec, tile0, user_emb, ldu, d, users, n_eval, tr_ptr, he_ptr, tid);
     if constexpr (kFull)
         eval_positives(t, pstage, uvec, item_emb, ldi, n_items, d, tr_idx, he_ptr, he_idx, pos_ws, pos_ws_off, tile0, warp, lane);
@@ -378,6 +401,10 @@ __global__ void __launch_bounds__(kEvalThreads, kFull ? 2 : 0) eval_rank_kernel(
         if (t.uid[u] < 0) continue;                                      // warp-uniform
         const int64_t g = tile0 + u;
         const int m = min(t.cnt[u], ks.kmax);                            // length of the hit list (batch_test.py:29-34)
+        if constexpr (kRec) {                                            // the ranked list is the whole output
+            eval_write_list(keys[u], m, ks.kmax, ranked + g * ldo, ranked_scores ? ranked_scores + g * ldo : nullptr, lane);
+            continue;
+        }
         const int64_t hb = he_ptr[t.uid[u]], he = he_ptr[t.uid[u] + 1];
         uint64_t H = 0ull;
         for (int half = 0; half < 2; ++half) {
@@ -564,14 +591,15 @@ __device__ __forceinline__ uint64_t* eval_sort_desc(uint64_t* a, uint64_t* s, in
     return a;
 }
 
-template <bool kFull>
+template <bool kFull, bool kRec = false>
 __global__ void __launch_bounds__(kEvalThreads, 1) eval_wide_kernel(
     const float* __restrict__ user_emb, int64_t ldu, const float* __restrict__ item_emb, int64_t ldi, int64_t n_items, int d,
     const int64_t* __restrict__ users, int64_t n_eval, const int64_t* __restrict__ tr_ptr, const int64_t* __restrict__ tr_idx,
     const int64_t* __restrict__ he_ptr, const int64_t* __restrict__ he_idx, const int32_t* __restrict__ ks, int n_ks, int kmax,
     int ksel, int cap, uint64_t* key_ws, int32_t* __restrict__ ranked, float* __restrict__ ranked_scores,
     int32_t* __restrict__ hits_out, double* __restrict__ per_user, float* __restrict__ scores_out, double* __restrict__ auc_out,
-    uint32_t* pos_ws, const int64_t* __restrict__ pos_ws_off) {
+    uint32_t* pos_ws, const int64_t* __restrict__ pos_ws_off, int64_t ldo) {
+    static_assert(!(kFull && kRec), "recommendation has no full mode");
     extern __shared__ __align__(16) unsigned char eval_smem[];
     float* uvec = reinterpret_cast<float*>(eval_smem);
     // candidate buffers: after the user vectors (8 d floats, a multiple of 16 bytes), or the CTA's workspace slot
@@ -631,6 +659,10 @@ __global__ void __launch_bounds__(kEvalThreads, 1) eval_wide_kernel(
             const int64_t g = tile0 + u;
             const int m = t.cnt[u];                                      // length of the hit list (batch_test.py:29-34)
             const uint64_t* sk = sorted[u];
+            if constexpr (kRec) {                                        // the ranked list is the whole output
+                eval_write_list(sk, m, kmax, ranked + g * ldo, ranked_scores ? ranked_scores + g * ldo : nullptr, lane);
+                continue;
+            }
             uint8_t* hitf = reinterpret_cast<uint8_t*>(sk == keys + (size_t)u * cap ? keys + (size_t)u * cap + ksel : keys + (size_t)u * cap);
             const int64_t hb = he_ptr[t.uid[u]], he = he_ptr[t.uid[u] + 1];
             int nh_all = 0;
@@ -741,7 +773,7 @@ static int eval_rank_launch(const float* user_emb, int64_t ldu, const float* ite
     const unsigned grid = (unsigned)((n_eval + kEvalUsers - 1) / kEvalUsers);
     eval_rank_kernel<kFull><<<grid, kEvalThreads, smem, (cudaStream_t)stream_>>>(
         user_emb, ldu, item_emb, ldi, n_items, d, users, n_eval, train_indptr, train_indices, held_indptr, held_indices, ks,
-        ranked, ranked_scores, hits, per_user, scores_out, auc_per_user, pos_ws, pos_ws_off);
+        ranked, ranked_scores, hits, per_user, scores_out, auc_per_user, pos_ws, pos_ws_off, (int64_t)ks.kmax);
     MMSSL_LAUNCH_OK();
     return 0;
 }
@@ -834,13 +866,54 @@ extern "C" int mmssl_eval_rank_wide(const float* user_emb, int64_t ldu, const fl
         eval_wide_kernel<true><<<(unsigned)p.grid, kEvalThreads, p.smem, st>>>(
             user_emb, ldu, item_emb, ldi, n_items, d, users, n_eval, train_indptr, train_indices, held_indptr, held_indices, ks_dev,
             n_ks, kmax, p.ksel, p.cap, p.ws_keys ? key_ws : nullptr, ranked, ranked_scores, hits, per_user, scores_out, auc_per_user,
-            pos_ws, pos_ws_off);
+            pos_ws, pos_ws_off, (int64_t)kmax);
     } else {
         MMSSL_CUDA(cudaFuncSetAttribute(eval_wide_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
         eval_wide_kernel<false><<<(unsigned)p.grid, kEvalThreads, p.smem, st>>>(
             user_emb, ldu, item_emb, ldi, n_items, d, users, n_eval, train_indptr, train_indices, held_indptr, held_indices, ks_dev,
             n_ks, kmax, p.ksel, p.cap, p.ws_keys ? key_ws : nullptr, ranked, ranked_scores, hits, per_user, scores_out, nullptr,
-            nullptr, nullptr);
+            nullptr, nullptr, (int64_t)kmax);
+    }
+    MMSSL_LAUNCH_OK();
+    return 0;
+}
+
+// Recommendation: the k <= 64 route is eval_rank_kernel's 512-key shared buffers, any larger k eval_wide_kernel's buffers with
+// the wide path's sizing (shared memory, else a key_ws slot per CTA) -- the routes and keys of mmssl_eval_rank / _wide with
+// Ks = [k], so the lists are the evaluator's bit for bit.
+extern "C" int64_t mmssl_recommend_workspace_bytes(int64_t n, int k, int64_t n_items, int d) {
+    return k <= kEvalMaxK ? 0 : mmssl_eval_wide_workspace_bytes(n, k, n_items, d);
+}
+
+extern "C" int mmssl_recommend_topk(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
+                                    const int64_t* users, int64_t n, const int64_t* excl_indptr, const int64_t* excl_indices, int k,
+                                    int64_t ldo, int32_t* ids, float* scores, uint64_t* key_ws, void* stream_) {
+    MMSSL_REQUIRE(d >= 4 && d <= 256 && (d & 3) == 0, "embedding width must be a multiple of 4, at most 256");
+    MMSSL_REQUIRE((ldi & 3) == 0 && aligned16(item_emb), "item table rows must be 16-byte aligned");
+    MMSSL_REQUIRE(n_items >= 0 && n_items < (1ll << 31), "bad item count");
+    MMSSL_REQUIRE(k >= 1 && k <= kEvalWideMaxK, "k must be in 1..2^26");
+    MMSSL_REQUIRE(ldo >= k, "ldo must be at least k");
+    MMSSL_REQUIRE(ids != nullptr && excl_indptr != nullptr && excl_indices != nullptr, "ids and the exclusion CSR are required");
+    if (n == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (k <= kEvalMaxK) {
+        EvalKs ks;
+        ks.n = 1;
+        ks.kmax = k;
+        for (int q = 0; q < kEvalMaxKs; ++q) ks.k[q] = 0;
+        ks.k[0] = k;
+        const size_t smem = sizeof(uint64_t) * kEvalUsers * kEvalCap + sizeof(float) * kEvalUsers * (size_t)d;
+        const unsigned grid = (unsigned)((n + kEvalUsers - 1) / kEvalUsers);
+        eval_rank_kernel<false, true><<<grid, kEvalThreads, smem, st>>>(
+            user_emb, ldu, item_emb, ldi, n_items, d, users, n, excl_indptr, excl_indices, nullptr, nullptr, ks, ids, scores, nullptr,
+            nullptr, nullptr, nullptr, nullptr, nullptr, ldo);
+    } else {
+        const EvalWidePlan p = eval_wide_plan(n, k, n_items, d);
+        MMSSL_REQUIRE(p.ws_keys == 0 || key_ws != nullptr, "key_ws (mmssl_recommend_workspace_bytes) is required");
+        MMSSL_CUDA(cudaFuncSetAttribute(eval_wide_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+        eval_wide_kernel<false, true><<<(unsigned)p.grid, kEvalThreads, p.smem, st>>>(
+            user_emb, ldu, item_emb, ldi, n_items, d, users, n, excl_indptr, excl_indices, nullptr, nullptr, nullptr, 0, k, p.ksel,
+            p.cap, p.ws_keys ? key_ws : nullptr, ids, scores, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, ldo);
     }
     MMSSL_LAUNCH_OK();
     return 0;

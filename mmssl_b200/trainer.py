@@ -173,6 +173,34 @@ class Trainer:
         outs, _ = hs.engine.forward(hs.P, hs.feats, hs.graphs, None, want_sumsq=False)       # model.eval(): no dropout
         return self.evaluator.test_torch(outs[0], outs[1], users_to_test, is_val)
 
+    _seen = None                                     # the "seen" exclusion CSR, built on first use
+
+    def recommender(self, k: int, exclude: str = "train"):
+        """(recommend.Recommender over the model's item table, the user table) of the eval-mode forward ``test`` runs (the full
+        step's current modality graphs), excluding "train" (what ``test`` masks) or "seen" (also the validation and test items).
+        ``recommend`` ranks with it; ``Recommender.export`` writes every user's list to files."""
+        from .recommend import EXCLUDE, Recommender, exclusion_rows
+        from .evaluate import _rows_to_csr
+        if exclude not in EXCLUDE:
+            raise ValueError(f"exclude must be one of {EXCLUDE}, not {exclude!r}")
+        if exclude == "train":
+            rows = self.evaluator.train
+        else:
+            if self._seen is None:
+                d = self.data
+                self._seen = _rows_to_csr(exclusion_rows(d.train_items, d.test_set, d.val_set, "seen"), self.n_users, self.device)
+            rows = self._seen
+        hs = self.step.hs
+        outs, _ = hs.engine.forward(hs.P, hs.feats, hs.graphs, None, want_sumsq=False)       # model.eval(): no dropout
+        return Recommender(outs[1], rows, k), outs[0]
+
+    def recommend(self, users, k: int, exclude: str = "train"):
+        """The top-k items of each of `users` the model has not been shown: (ids [n, k] int64, scores [n, k] fp32) on the device,
+        -1 past the end of a short list.  exclude="train" masks what ``test`` masks, so the lists are the evaluator's ranked lists
+        with Ks = [k]; "seen" also masks the validation and test items (recommend.py)."""
+        rec, user_table = self.recommender(k, exclude)
+        return rec.topk(user_table, users)
+
     def sample(self):
         if self.sampler == "device":
             self._dev_sampler.sample_into(self._triples, step=self._n_sampled)

@@ -1,0 +1,116 @@
+"""Export the top-k recommendations of every user of a trained model (mmssl_b200/recommend.py).
+
+    python tools/recommend.py DATA --checkpoint run.ckpt --k 20 [--exclude train|seen] --out DIR [--chunk N]
+        DATA: a dataset directory in the reference format (dataset.ReferenceDataset); run.ckpt: a ``Trainer.save`` file of a run on
+        it.  Rebuilds the Trainer with the checkpoint's shape, loads it and writes DIR/{ids,scores,users}.npy + manifest.json.
+    python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tools/recommend.py --sharded CKPT_DIR \\
+        --shards SHARD_DIR --k 20 [--exclude train|seen] --out DIR
+        CKPT_DIR: a row-sharded checkpoint (``RowShardedHotStep.save``, any world size); SHARD_DIR: ``dataset.write_shards`` output
+        of its dataset.  Each rank loads its rows (resharded to N), runs the eval-mode forward and writes
+        DIR/rankRRRRR-of-WWWWW.{ids,scores,users}.npy + .json for the users of its block.
+    Neither checkpoint kind stores id_cat_rate / model_cat_rate, which shape the eval-mode forward: a run trained with other
+    values than the defaults (0.36 / 0.55) needs --id-cat-rate / --model-cat-rate, in both modes.
+
+``recommend.read(DIR)`` returns (users, ids, scores) of either layout.  Prints one JSON line (rank 0)."""
+import argparse
+import json
+import os
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+import torch.distributed as dist  # noqa: E402
+
+from mmssl_b200 import checkpoint, recommend  # noqa: E402
+
+
+def one_gpu(a, dev):
+    from mmssl_b200.dataset import ReferenceDataset
+    from mmssl_b200.trainer import Trainer, TrainerArgs
+    st = checkpoint.load(a.checkpoint, kinds=("trainer",))
+    meta, tr = st["meta"], st["trainer"]
+    d = int(meta["embed_size"])
+    args = TrainerArgs(dataset=os.path.basename(os.path.normpath(a.data)), embed_size=d, batch_size=int(meta["batch_size"]),
+                       head_num=int(meta["head_num"]), weight_size=str([d] * int(meta["n_layers"])), id_cat_rate=a.id_cat_rate,
+                       model_cat_rate=a.model_cat_rate)
+    if tr["sampler"] == "device":
+        args.seed = int(tr["sampler_seed"])
+    del st
+    ds = ReferenceDataset.load(a.data)
+    t = Trainer(ds, args, device=dev, sampler=tr["sampler"], log=None)
+    t.load(a.checkpoint)
+    rec, user_table = t.recommender(a.k, a.exclude)                 # what Trainer.recommend ranks with
+    n = rec.export(user_table, np.arange(t.n_users, dtype=np.int64), a.out, chunk=a.chunk)
+    return dict(users=n, items=t.n_items)
+
+
+def sharded(a, dev, rank, world):
+    from mmssl_b200.dataset import ShardedDataset
+    from mmssl_b200.engine import P_EI, P_EU
+    from mmssl_b200.hotstep import HotStepConfig
+    from mmssl_b200.rowshard_step import RowShardedHotStep, shard_problem_from_disk
+    st = checkpoint.read_sharded(a.sharded, world, rank)
+    meta = st["meta"]
+    sh = ShardedDataset.open(a.shards, rank, world)
+    if (sh.n_users, sh.n_items) != (meta["n_users"], meta["n_items"]):
+        raise SystemExit(f"{a.shards} holds {sh.n_users} x {sh.n_items}, the checkpoint {meta['n_users']} x {meta['n_items']}")
+    # parameters of the right shapes (the load below overwrites every value): the replicated ones from the file, the two tables
+    # as full-height placeholders that shard_problem_from_disk cuts into this rank's blocks
+    P = {k: v for k, v in st["model"].items() if k not in (P_EU, P_EI)}
+    P[P_EU] = torch.zeros(meta["n_users"], meta["embed_size"])
+    P[P_EI] = torch.zeros(meta["n_items"], meta["embed_size"])
+    Pl, fl, gl, pu, pi = shard_problem_from_disk(a.shards, P, rank, world, dev)
+    B = int(meta["batch_size"])
+    cfg = HotStepConfig(embed_size=int(meta["embed_size"]), n_layers=int(meta["n_layers"]), head_num=int(meta["head_num"]), batch_size=B,
+                        id_cat_rate=a.id_cat_rate, model_cat_rate=a.model_cat_rate)
+    step = RowShardedHotStep(Pl, fl, gl, cfg, B, pu, pi, rank)
+    del st, P
+    step.load(a.sharded)
+    u_f, i_f = step.final_embeddings()
+    rec = recommend.ShardedRecommender.from_shards(sh, a.k, a.exclude, device=dev)
+    n = rec.export(u_f, i_f, np.arange(sh.n_users, dtype=np.int64), a.out, chunk=a.chunk)
+    return dict(users=sh.n_users, items=sh.n_items, rows_written_by_rank0=n)
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("data", nargs="?", help="dataset directory (reference format), with --checkpoint")
+    ap.add_argument("--checkpoint", help="a Trainer.save file")
+    ap.add_argument("--sharded", help="a row-sharded checkpoint directory (under torch.distributed.run)")
+    ap.add_argument("--shards", help="dataset.write_shards output of the dataset, with --sharded")
+    ap.add_argument("--k", type=int, default=20)
+    ap.add_argument("--exclude", choices=recommend.EXCLUDE, default="train")
+    ap.add_argument("--out", required=True)
+    ap.add_argument("--chunk", type=int, default=1 << 16, help="users ranked per launch (bounds the device memory)")
+    # both rates shape the eval-mode forward and neither checkpoint kind stores them: give the trained run's values
+    ap.add_argument("--id-cat-rate", type=float, default=0.36, help="the run's id_cat_rate (not in its checkpoint; default 0.36)")
+    ap.add_argument("--model-cat-rate", type=float, default=0.55, help="the run's model_cat_rate (not in its checkpoint; default 0.55)")
+    a = ap.parse_args(argv)
+    if bool(a.sharded) == bool(a.checkpoint) or (a.sharded and not a.shards) or (a.checkpoint and not a.data):
+        ap.error("give DATA --checkpoint FILE, or --sharded DIR --shards DIR")
+    rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
+    torch.cuda.set_device(local)
+    dev = torch.device("cuda", local)
+    t0 = time.perf_counter()
+    if a.sharded:
+        own = world > 1 and not dist.is_initialized()       # (a caller may have set up the process group already)
+        if own:
+            dist.init_process_group("nccl", device_id=dev)
+        res = sharded(a, dev, rank, world)
+        if world > 1:
+            dist.barrier()
+        if own:
+            dist.destroy_process_group()
+    else:
+        res = one_gpu(a, dev)
+    res.update(k=a.k, exclude=a.exclude, n_gpus=world, out=os.path.abspath(a.out), seconds=round(time.perf_counter() - t0, 2))
+    if rank == 0:
+        print(json.dumps(res))
+    return res
+
+
+if __name__ == "__main__":
+    main()
