@@ -461,9 +461,10 @@ class RowShardedHotStep:
         elif self.pu.world > 1:
             dist.all_reduce(self._flat, op=dist.ReduceOp.SUM, group=self.group)
         if self.pu.world > 1:
-            feat = self._flat[self._feat_slot]
-            self.out5[0] += feat - self.out5[3]
-            self.out5[3] = feat
+            # the total is formed again from the all-reduced feat_reg, in loss_assemble's order, from terms that are equal on
+            # every rank: `total += feat - feat_local` rounded differently on each rank, and the losses differed in the last bit
+            self.out5[3] = self._flat[self._feat_slot]
+            self.out5[0] = self.out5[1] + self.out5[2] + self.out5[3] + cfg.cl_rate * self.out5[4]
         if self.optimizer_step:
             ops.step_tick(self.step_dev)
             keys = list(LIVE)
