@@ -189,6 +189,9 @@ int mmssl_combine_bwd(const float* g, int64_t ldg, const float* a, int64_t lda, 
 /* t = y * (alpha*g - <alpha*g, y>)  (softmax backward for one tensor) */
 int mmssl_softmax_bwd(const float* y, int64_t ldy, const float* g, int64_t ldg, int64_t n, int d, float alpha,
                       float* t, int64_t ldt, void* stream);
+/* out = x / max(|x|_2, 1e-12) row by row (F.normalize; a zero row stays zero), strided [n, d] rows at the six embedding widths.
+ * A row's result depends on that row only, not on n or the launch shape (the unit tables of item-to-item similarity). */
+int mmssl_unit_rows(const float* x, int64_t ldx, int64_t n, int d, float* out, int64_t ldo, void* stream);
 /* y = alpha * (alpha_dev ? *alpha_dev : 1) * x + beta * y, strided rows (alpha_dev: optional device scalar) */
 int mmssl_axpby(const float* x, int64_t ldx, int64_t n, int d, float alpha, const float* alpha_dev, float beta, float* y, int64_t ldy, void* stream);
 /* dropout apply: y = x * mask (mask holds 0 or 1/(1-p)) ; mask may be NULL (copy) */

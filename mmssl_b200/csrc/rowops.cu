@@ -5,6 +5,7 @@
 //   combine      Models.py:213-218   uf = mean_k(u_k) + model_cat_rate*(normalize(Uv)+normalize(Ut))
 //                                    (+ the sums of squares main.py:252-257 needs, for free)
 //   softmax_bwd  backward of Models.py:203-204
+//   unit_rows    out = normalize(x): the unit tables of item-to-item similarity (similar.py)
 #include "common.cuh"
 #include "../../include/mmssl_b200.h"
 
@@ -210,6 +211,21 @@ __global__ void __launch_bounds__(256) softmax_bwd_kernel(const float* __restric
     store_row<G, C>(gv, t, ldt, ix);
 }
 
+// out = x / max(|x|, eps), F.normalize with id_fuse's norm: one lane group per row, so a row's bits depend on that row only
+template <int G, int C>
+__global__ void __launch_bounds__(256) unit_rows_kernel(const float* __restrict__ x, int64_t ldx, int64_t n,
+                                                        float* __restrict__ out, int64_t ldo) {
+    pdl_wait();
+    RowIdx<G, C> ix;
+    if (ix.row >= n) return;
+    float4 v[C];
+    load_row<G, C>(v, x, ldx, ix);
+    const float inv = 1.f / fmaxf(sqrtf(row_dot<G, C>(v, v, ix.mask)), kNormEps);
+#pragma unroll
+    for (int c = 0; c < C; ++c) v[c] = scale4(v[c], inv);
+    store_row<G, C>(v, out, ldo, ix);
+}
+
 // ---- plain element-wise passes over strided [n, d] matrices (d % 4 == 0) ----
 __global__ void axpby_kernel(const float* __restrict__ x, int64_t ldx, int64_t n, int d4, float alpha,
                              const float* __restrict__ alpha_dev, float beta, float* __restrict__ y, int64_t ldy) {
@@ -364,6 +380,17 @@ extern "C" int mmssl_softmax_bwd(const float* y, int64_t ldy, const float* g, in
     if (n == 0) return 0;
     return dispatch_width(d, [&](auto G, auto C) {
         MMSSL_CUDA_LAUNCH((softmax_bwd_kernel<decltype(G)::value, decltype(C)::value>), dim3(row_blocks(n, decltype(G)::value)), dim3(256), 0, st, y, ldy, g, ldg, n, alpha, t, ldt);
+        MMSSL_LAUNCH_OK();
+        return 0;
+    }, __func__);
+}
+
+extern "C" int mmssl_unit_rows(const float* x, int64_t ldx, int64_t n, int d, float* out, int64_t ldo, void* stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    MMSSL_REQUIRE(ROW_ALIGN_OK(x, ldx) && ROW_ALIGN_OK(out, ldo), "alignment");
+    if (n == 0) return 0;
+    return dispatch_width(d, [&](auto G, auto C) {
+        MMSSL_CUDA_LAUNCH((unit_rows_kernel<decltype(G)::value, decltype(C)::value>), dim3(row_blocks(n, decltype(G)::value)), dim3(256), 0, st, x, ldx, n, out, ldo);
         MMSSL_LAUNCH_OK();
         return 0;
     }, __func__);

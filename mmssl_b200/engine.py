@@ -173,10 +173,13 @@ class Engine:
         return torch.empty(*shape, dtype=torch.float32, device=dev)
 
     # ------------------------------------------------------------------ projection
-    def _project(self, P, feats, masks, ys, wait_for=None):
+    def _project(self, P, feats, masks, ys, wait_for=None, plan_rows=None):
         """X = F W^T + b, then the dropout mask, for image and text (Models.py:173-174).  Tensor cores: both GEMMs in ONE
         grouped persistent launch (the feature streams of 118 + 30 MB at Baby share one balanced wave), then the two
-        split-K epilogues.  `wait_for`: a branch whose work (the mask draws) the epilogues wait for; the GEMM does not."""
+        split-K epilogues.  `wait_for`: a branch whose work (the mask draws) the epilogues wait for; the GEMM does not.
+        `plan_rows`: the row count the K split is planned for (default: the rows projected).  The split fixes the order in which
+        a row's products are summed, so rows projected in launches of different heights under one plan_rows get the same
+        bits: a rank's item block, or a few feature rows, projects as the whole catalogue does (similar.py)."""
         d = self.d
         dev = ys[0].device
         ws, bs = (P[P_WV], P[P_WT]), (P[P_BV], P[P_BT])
@@ -185,7 +188,11 @@ class Engine:
             self._fork(dev, "fork2", lambda: self._project_simt(ws[0], bs[0], feats[0], masks[0], ys[0]),
                        lambda: self._project_simt(ws[1], bs[1], feats[1], masks[1], ys[1]))
             return
-        splits, floats = ops.gemm_bf16x3_group_plan([(fs.n_items, d, fs.dim) for fs in feats], self.proj_max_ctas)
+        if plan_rows is None:
+            splits, floats = ops.gemm_bf16x3_group_plan([(fs.n_items, d, fs.dim) for fs in feats], self.proj_max_ctas)
+        else:
+            splits, _ = ops.gemm_bf16x3_group_plan([(int(plan_rows), d, fs.dim) for fs in feats], self.proj_max_ctas)
+            floats = [sk * fs.n_items * d for sk, fs in zip(splits, feats)]
         parts = self._new(sum(floats), dev=dev).split(floats)
         probs = []
         for w, fs, sk, part in zip(ws, feats, splits, parts):

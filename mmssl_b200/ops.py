@@ -201,6 +201,16 @@ def softmax_bwd(y, g, alpha: float, out):
     return out
 
 
+def unit_rows(x, out=None):
+    """out = x / max(|x|, 1e-12) row by row (F.normalize); a row's bits depend on that row only."""
+    lib = _lib_()
+    n, d = x.shape
+    if out is None:
+        out = torch.empty(n, d, dtype=torch.float32, device=x.device)
+    _lib.check(lib.mmssl_unit_rows(ptr(x), _ld(x), n, d, ptr(out), _ld(out), stream()))
+    return out
+
+
 def axpby(x, alpha: float, beta: float, y, alpha_dev=None):
     lib = _lib_()
     n, d = x.shape

@@ -35,6 +35,8 @@ from .parallel import RowPartition, all_gather_rows
 
 EXCLUDE = ("train", "seen")
 FILES = ("ids", "scores", "users")
+FORMAT = "mmssl_b200.recommend.v1"
+QUERY_FILES = ("users", "items")            # the row-id file of a recommendation / a similar-items (similar.py) export
 MANIFEST = "manifest.json"
 _RANK_MANIFEST = re.compile(r"rank(\d{5})-of-(\d{5})\.json")
 
@@ -98,18 +100,23 @@ class _Files:
     are removed (from then on the directory holds no committed export that the new files could mix with); ``commit`` renames
     the files over their final names and then writes the export's manifest, which is what makes them readable."""
 
-    def __init__(self, out_dir: str, prefix: str, n: int, k: int, export_id: int, stale):
+    def __init__(self, out_dir: str, prefix: str, n: int, k: int, export_id: int, stale, query: str = "users", meta=None):
+        """query: the name of the file of row ids ("users" here, "items" for similar.py); meta: the manifest's format and
+        whatever else it records (default: a recommendation export).  The other kind's row-id file under the same prefix is
+        removed with the stale manifests: it belongs to an export this one supersedes and would be left behind."""
         os.makedirs(out_dir, exist_ok=True)
+        stale = list(stale) + [f"{prefix}{q}.npy" for q in QUERY_FILES if q != query]
         for name in stale:
             try:
                 os.remove(os.path.join(out_dir, name))
             except FileNotFoundError:
                 pass
-        self.final = {f: os.path.abspath(os.path.join(out_dir, f"{prefix}{f}.npy")) for f in FILES}
+        self.files = ("ids", "scores", query)
+        self.final = {f: os.path.abspath(os.path.join(out_dir, f"{prefix}{f}.npy")) for f in self.files}
         self.manifest = os.path.abspath(os.path.join(out_dir, _manifest_name(prefix)))
-        self.meta = dict(format="mmssl_b200.recommend.v1", export=int(export_id), n=int(n), k=int(k))
+        self.meta = dict(meta or dict(format=FORMAT), export=int(export_id), n=int(n), k=int(k))
         self.tmp, self.arr = {}, {}
-        spec = {"ids": (np.int32, (n, k)), "scores": (np.float32, (n, k)), "users": (np.int64, (n,))}
+        spec = {"ids": (np.int32, (n, k)), "scores": (np.float32, (n, k)), query: (np.int64, (n,))}
         try:
             for f, (dt, shape) in spec.items():
                 self.tmp[f] = _tmp_path(self.final[f])
@@ -123,14 +130,14 @@ class _Files:
             raise
 
     def commit(self) -> None:
-        for f in FILES:
+        for f in self.files:
             a = self.arr.pop(f, None)
             if a is not None:
                 a.flush()
                 del a
             with open(self.tmp[f], "rb+") as fh:
                 os.fsync(fh.fileno())
-        for f in FILES:
+        for f in self.files:
             os.replace(self.tmp[f], self.final[f])
         tmp = _tmp_path(self.manifest)
         try:
@@ -239,15 +246,16 @@ class Recommender:
         return self._export(ua, ids_np, ids_np, out_dir, chunk, "", _new_export_id(), [MANIFEST] + list(ranks.values()))
 
     def _export(self, ua, ids_np: np.ndarray, names: np.ndarray, out_dir: str, chunk: int, prefix: str, export_id: int,
-                stale) -> int:
-        """export() of the rows ids_np of ua; ``users.npy`` gets `names` (the global ids of a row-sharded rank's local rows)."""
+                stale, query: str = "users", meta=None) -> int:
+        """export() of the rows ids_np of ua; ``users.npy`` gets `names` (the global ids of a row-sharded rank's local rows).
+        query / meta: see _Files."""
         if chunk < 1:
             raise ValueError("chunk must be >= 1")
         n = ids_np.size
-        files = _Files(out_dir, prefix, n, self.k, export_id, stale)
+        files = _Files(out_dir, prefix, n, self.k, export_id, stale, query, meta)
         try:
             if n:
-                files.arr["users"][:] = names
+                files.arr[query][:] = names
                 self._export_chunks(ua, ids_np, files.arr, chunk)
             files.commit()
         except BaseException:
@@ -300,28 +308,47 @@ def _new_export_id() -> int:
     return int.from_bytes(os.urandom(8), "little") >> 2
 
 
-def _load_set(out_dir: str, prefix: str, meta: dict):
-    arrs = {f: np.load(os.path.join(out_dir, f"{prefix}{f}.npy"), mmap_mode="r") for f in FILES}
+def _load_set(out_dir: str, prefix: str, meta: dict, query: str = "users"):
+    arrs = {f: np.load(os.path.join(out_dir, f"{prefix}{f}.npy"), mmap_mode="r") for f in ("ids", "scores", query)}
     n, k = meta["n"], meta["k"]
-    if arrs["ids"].shape != (n, k) or arrs["scores"].shape != (n, k) or arrs["users"].shape != (n,):
+    if arrs["ids"].shape != (n, k) or arrs["scores"].shape != (n, k) or arrs[query].shape != (n,):
         raise ValueError(f"{out_dir}: the {prefix}*.npy files do not have the shapes their manifest names")
     return arrs
+
+
+# the readers of the export formats that share the file logic above: a directory of one kind is refused by the other's reader
+READERS = {FORMAT: "recommendations (mmssl_b200.recommend.read)",
+           "mmssl_b200.similar.v1": "similar items (mmssl_b200.similar.read)"}
+
+
+def _check_format(out_dir: str, meta: dict, fmt: str) -> None:
+    got = meta.get("format", fmt)
+    if got != fmt:
+        raise ValueError(f"{out_dir}: holds an export of {READERS.get(got, repr(got))}, not of {READERS[fmt]}")
 
 
 def read(out_dir: str) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """(users [n] int64, ids [n, k] int32, scores [n, k] fp32) of the committed export in out_dir.  One-GPU layout (manifest.json):
     the files as written (memory-mapped), rows in the order the users were listed.  Row-sharded layout (rankRRRRR-of-WWWWW.json):
     every rank's rows, in ascending user order (the listed order among equal ids); every rank's manifest must be present and all
-    must name the same export, so the files of an export that did not finish on every rank are never read as a whole."""
+    must name the same export, so the files of an export that did not finish on every rank are never read as a whole.  A
+    similar-items export (similar.py) is refused."""
+    return _read(out_dir, "users", FORMAT, "recommendation")
+
+
+def _read(out_dir: str, query: str, fmt: str, what: str):
+    """read() of the exports whose row-id file is ``<query>.npy`` and whose manifests name format `fmt`."""
     one, ranks = _manifests(out_dir)
     if not one and not ranks:
-        raise ValueError(f"{out_dir}: no committed recommendation export (manifest.json or rankRRRRR-of-WWWWW.json)")
+        raise ValueError(f"{out_dir}: no committed {what} export (manifest.json or rankRRRRR-of-WWWWW.json)")
     if one and ranks:
         raise ValueError(f"{out_dir}: holds a one-GPU and a row-sharded export: remove one")
     if one:
         with open(os.path.join(out_dir, MANIFEST)) as fh:
-            arrs = _load_set(out_dir, "", json.load(fh))
-        return arrs["users"], arrs["ids"], arrs["scores"]
+            meta = json.load(fh)
+        _check_format(out_dir, meta, fmt)
+        arrs = _load_set(out_dir, "", meta, query)
+        return arrs[query], arrs["ids"], arrs["scores"]
     worlds = sorted({w for _, w in ranks})
     if len(worlds) > 1:
         raise ValueError(f"{out_dir}: exports of several world sizes {worlds}: remove all but one")
@@ -333,13 +360,24 @@ def read(out_dir: str) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     for r in range(w):
         with open(os.path.join(out_dir, ranks[(r, w)])) as fh:
             metas.append(json.load(fh))
+        _check_format(out_dir, metas[-1], fmt)
     if len({m["export"] for m in metas}) != 1 or len({m["k"] for m in metas}) != 1:
         raise ValueError(f"{out_dir}: the rank files of world size {w} belong to different exports")
-    parts = [_load_set(out_dir, _rank_prefix(r, w), metas[r]) for r in range(w)]
-    users = np.concatenate([p["users"] for p in parts])
-    order = np.argsort(users, kind="stable")
-    return (users[order], np.concatenate([p["ids"] for p in parts])[order],
+    parts = [_load_set(out_dir, _rank_prefix(r, w), metas[r], query) for r in range(w)]
+    queries = np.concatenate([p[query] for p in parts])
+    order = np.argsort(queries, kind="stable")
+    return (queries[order], np.concatenate([p["ids"] for p in parts])[order],
             np.concatenate([p["scores"] for p in parts])[order])
+
+
+def _sharded_stale(out_dir: str, rank: int, world: int):
+    """The manifests a row-sharded export of (rank, world) removes before it writes: the rank's own, and on rank 0 those of a
+    one-GPU export and of other world sizes."""
+    stale = [_manifest_name(_rank_prefix(rank, world))]
+    if rank == 0:
+        _, ranks = _manifests(out_dir)
+        stale += [MANIFEST] + [name for (_, w), name in ranks.items() if w != world]
+    return stale
 
 
 class ShardedRecommender:
@@ -421,10 +459,7 @@ class ShardedRecommender:
         of rows written."""
         ids = self.check_users(users)
         prefix = _rank_prefix(self.rank_id, self.pu.world)
-        stale = [_manifest_name(prefix)]
-        if self.rank_id == 0:
-            _, ranks = _manifests(out_dir)
-            stale += [MANIFEST] + [name for (_, w), name in ranks.items() if w != self.pu.world]
+        stale = _sharded_stale(out_dir, self.rank_id, self.pu.world)
         export_id = self.export_id()
         rec = self.local(self.gather_items(i_local))
         mine = ids[self.mine(ids)]
@@ -432,10 +467,15 @@ class ShardedRecommender:
                            stale)
 
     def export_id(self) -> int:
-        """Collective.  A fresh random id, the same on every rank: rank 0's draw (the only non-zero term of a sum)."""
-        export_id = _new_export_id() if self.rank_id == 0 else 0
-        if self.pu.world > 1:
-            t = torch.tensor([export_id], dtype=torch.int64, device=self.device)
-            dist.all_reduce(t, group=self.group)
-            export_id = int(t.item())
-        return export_id
+        """Collective.  A fresh random id, the same on every rank."""
+        return shared_export_id(self.rank_id, self.pu.world, self.device, self.group)
+
+
+def shared_export_id(rank: int, world: int, device, group=None) -> int:
+    """Collective.  A fresh random id, the same on every rank: rank 0's draw (the only non-zero term of a sum)."""
+    export_id = _new_export_id() if rank == 0 else 0
+    if world > 1:
+        t = torch.tensor([export_id], dtype=torch.int64, device=device)
+        dist.all_reduce(t, group=group)
+        export_id = int(t.item())
+    return export_id

@@ -493,6 +493,18 @@ class RowShardedHotStep:
         self.n_gathers, self.gathered_bytes, self.n_reduce_scatters = counters
         return outs[0], outs[1]
 
+    def projections(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The eval-mode modality projections Xv = Fv Wv^T + bv, Xt = Ft Wt^T + bt (Models.py:173-174, no dropout) of the rank's
+        padded [block, d] item rows, fresh tensors.  Row-local, so no collective: the rank's feature rows and the replicated
+        weights suffice.  The K split is planned for the whole catalogue (Engine._project's plan_rows), so every real row has
+        the bits of the one-GPU projection of the same parameters.  Writes nothing a step or a captured step reads (the
+        outputs are allocated here; the split-K partials are scratch).  Padding rows hold the bias."""
+        d, dev = self.cfg.embed_size, self.idx.device
+        x = torch.empty(self.pi.block, 2 * d, dtype=torch.float32, device=dev)
+        xv, xt = x[:, :d], x[:, d:]
+        self.engine._project(self.P, self.feats, (None, None), (xv, xt), plan_rows=self.pi.n)
+        return xv, xt
+
     def test(self, evaluator, users_to_test, is_val: bool) -> Dict[str, object]:
         """Collective.  ``Trainer.test`` of the row-sharded model: ``evaluator`` is this rank's ``evaluate.ShardedEvaluator``;
         returns its ``test_torch`` result, identical on every rank."""

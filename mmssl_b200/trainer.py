@@ -201,6 +201,24 @@ class Trainer:
         rec, user_table = self.recommender(k, exclude)
         return rec.topk(user_table, users)
 
+    def similar(self, k: int, space: str = "model"):
+        """similar.SimilarItems over the table of `space` of the eval-mode model ``test`` and ``recommender`` use: the final item
+        table ("model", from the same forward, with the full step's current modality graphs) or a modality projection ("image",
+        "text").  ``similar_items`` / ``similar_to_features`` rank with it; ``SimilarItems.export`` writes every item's list."""
+        from .similar import SimilarItems
+        hs = self.step.hs
+        return SimilarItems.from_model(hs.engine, hs.P, hs.feats, hs.graphs, k, space)
+
+    def similar_items(self, items, k: int, space: str = "model"):
+        """The k catalogue items most similar (cosine) to each of `items` in `space`, the item itself left out: (ids [n, k] int64,
+        scores [n, k] fp32) on the device, -1 past the end of a short list (similar.py)."""
+        return self.similar(k, space).topk(items)
+
+    def similar_to_features(self, image_feats, text_feats, k: int, space: str = "image"):
+        """The k catalogue items most similar to each of m new items given by their feature rows (image [m, Dv], text [m, Dt]),
+        projected with the trained weights, in space "image" or "text"."""
+        return self.similar(k, space).topk_features(image_feats, text_feats)
+
     def sample(self):
         if self.sampler == "device":
             self._dev_sampler.sample_into(self._triples, step=self._n_sampled)
