@@ -8,7 +8,9 @@
 // per-slot keys (select_pass_kernel and below), exact for any batch up to n_exist.
 // One CTA (batch <= 1024).  Distinctness without atomics races: rounds of "draw, atomicMin-claim,
 // check" -- the winner of a claim is the smallest thread id, so the result depends only on
-// (seed, step), never on scheduling; the claim table cleans itself up.  Counter-based RNG
+// (seed, step), never on scheduling; the claim table cleans itself up.  Threads the 64 rounds leave unserved (batch close to
+// n_exist) take the free slots of one sweep over the claim table (the claim finish), so the users are distinct at every
+// batch <= n_exist.  Negatives: after 4096 rejected draws, a uniform draw from the row's complement.  Counter-based RNG
 // (splitmix64 of (seed, step, thread, draw)), so the kernel is replayable inside a CUDA graph with
 // the step number read from device memory.
 // Row-sharded runs (ShardedTripleSampler): the same kernels with an owned slot range -- every rank selects the slots over the
@@ -34,6 +36,10 @@ __device__ __forceinline__ uint32_t rnd32(uint64_t seed, uint32_t step, uint32_t
 // unbiased enough for sampling: 32-bit multiply-shift range reduction
 __device__ __forceinline__ uint32_t below(uint32_t r, uint32_t n) { return (uint32_t)(((uint64_t)r * n) >> 32); }
 
+constexpr int kClaimRounds = 64;                        // claim-by-minimum rounds before the claim finish
+constexpr int kNegTries = 4096;                         // rejection draws of a negative before the complement draw
+constexpr uint64_t kFinishStream = 0xBB67AE8584CAA73Bull;   // the claim finish's start slot, apart from the per-thread draws
+
 // Triple t of the batch for the user of `slot`: one uniform positive from the user's row, one uniform negative rejected while it
 // is in the row; `draw` is the next unused draw number of thread t.  Shared by both sampler paths.
 // The rows are those of one block of users: the user of slot s is row0 + exist[s - slot_lo], whose row is indptr / indices of
@@ -49,14 +55,27 @@ __device__ __forceinline__ void draw_triple(const int64_t* __restrict__ indptr, 
     const uint32_t deg = (uint32_t)(e - b);
     const int64_t p = indices[b + below(rnd32(seed, step, t, draw++), deg)];
     int64_t ng = 0;
-    for (int tries = 0; tries < 4096; ++tries) {
+    bool in_row = true;
+    for (int tries = 0; tries < kNegTries && in_row; ++tries) {
         ng = below(rnd32(seed, step, t, draw++), (uint32_t)n_items);
         int64_t lo = b, hi = e;             // binary search in the (sorted) row
         while (lo < hi) {
             const int64_t mid = (lo + hi) >> 1;
             if ((int64_t)indices[mid] < ng) lo = mid + 1; else hi = mid;
         }
-        if (!(lo < e && (int64_t)indices[lo] == ng)) break;
+        in_row = lo < e && (int64_t)indices[lo] == ng;
+    }
+    if (in_row && (int64_t)deg < n_items) {
+        // A dense row rejected every try: the j-th item missing from the row, uniform over the complement, so the mixture with
+        // the rejection draws stays uniform.  Items below indices[b + m] missing from the row: indices[b + m] - m (sorted,
+        // distinct), so the answer is j + (number of row items below it) = j + (first m with indices[b + m] - m > j).
+        const int64_t j = below(rnd32(seed, step, t, draw++), (uint32_t)(n_items - deg));
+        int64_t lo = 0, hi = deg;
+        while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if ((int64_t)indices[b + mid] - mid <= j) lo = mid + 1; else hi = mid;
+        }
+        ng = j + lo;
     }
     users[t] = row0 + r; pos[t] = p; neg[t] = ng;
 }
@@ -74,6 +93,24 @@ __device__ __forceinline__ void draw_or_zero(const int64_t* __restrict__ indptr,
     draw_triple(indptr, indices, exist, slot, kOwned ? slot_lo : 0, kOwned ? row0 : 0, n_items, seed, step, t, draw, users, pos, neg);
 }
 
+// Threads of the block below this one whose `pred` holds (a block-wide exclusive count); `*total` (if given) = all of them.
+// Every thread of the block calls it; warp_count is free again on return.
+__device__ __forceinline__ int block_count_before(bool pred, int* warp_count, int* total) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, warps = (int)(blockDim.x >> 5);
+    const unsigned m = __ballot_sync(0xffffffffu, pred);
+    if (lane == 0) warp_count[w] = __popc(m);
+    __syncthreads();
+    int before = 0, all = 0;
+    for (int k = 0; k < warps; ++k) {
+        const int c = warp_count[k];
+        before += k < w ? c : 0;
+        all += c;
+    }
+    __syncthreads();
+    if (total) *total = all;
+    return before + __popc(m & ((1u << lane) - 1u));
+}
+
 template <typename IdxT, bool kOwned>
 __global__ void __launch_bounds__(1024) sample_triples_kernel(const int64_t* __restrict__ indptr,
                                                               const IdxT* __restrict__ indices,
@@ -83,6 +120,8 @@ __global__ void __launch_bounds__(1024) sample_triples_kernel(const int64_t* __r
                                                               int32_t* __restrict__ claim, int64_t* __restrict__ users,
                                                               int64_t* __restrict__ pos, int64_t* __restrict__ neg) {
     __shared__ int pending;
+    __shared__ int warp_count[32];
+    __shared__ int32_t given[1024];         // claim finish: the slot of the r-th thread still pending
     const int t = threadIdx.x;
     const uint32_t step = (uint32_t)(step_dev ? *step_dev : step_host);
     const bool with_replacement = batch > n_exist;
@@ -92,7 +131,8 @@ __global__ void __launch_bounds__(1024) sample_triples_kernel(const int64_t* __r
     if (with_replacement && !done) { slot = below(rnd32(seed, step, t, draw++), (uint32_t)n_exist); done = true; }
     // ---- distinct users: rounds of claim-by-minimum ----
     // claim[x]: INT_MAX = free, -1 = taken in an earlier round, otherwise the smallest contender id.
-    for (int round = 0; round < 64; ++round) {
+    int left = 0;
+    for (int round = 0; round < kClaimRounds; ++round) {
         if (t == 0) pending = 0;
         __syncthreads();
         int64_t cand = -1;
@@ -107,14 +147,37 @@ __global__ void __launch_bounds__(1024) sample_triples_kernel(const int64_t* __r
             if (!won) atomicAdd(&pending, 1);
         }
         __syncthreads();
-        const int left = pending;              // read before thread 0 may reset it for the next round
+        left = pending;                        // read before thread 0 may reset it for the next round
         if (won) { slot = cand; done = true; claim[cand] = -1; }
         __syncthreads();
         if (left == 0) break;
     }
-    if (t < batch && !with_replacement && slot >= 0) claim[slot] = 0x7fffffff;   // leave the table clean
+    // ---- claim finish (batch close to n_exist: the rounds are a coupon collector whose tail outlasts them) ----
+    // One sweep over the claim table from a random start slot, cyclically: the free slots are handed out in that order to the
+    // pending threads in thread order; it stops as soon as every pending thread has one, and at the latest after n_exist slots,
+    // which hold at least `left` free ones (batch <= n_exist).  A uniform start keeps the batch invariant under a rotation of the
+    // slots.  Runs only when the rounds did not finish (`left` is the same in every thread), so other batches keep their bits.
+    if (left > 0) {
+        const int64_t start = below(rnd32(seed ^ kFinishStream, step, 0, 0), (uint32_t)n_exist);
+        int served = 0;
+        for (int64_t c = 0; c < n_exist && served < left; c += blockDim.x) {
+            int64_t x = c + t;
+            bool free = false;
+            if (x < n_exist) {
+                x += start;
+                if (x >= n_exist) x -= n_exist;
+                free = claim[x] == 0x7fffffff;
+            }
+            int found;
+            const int at = served + block_count_before(free, warp_count, &found);
+            if (free && at < left) given[at] = (int32_t)x;
+            served += found;
+        }
+        const int rank = block_count_before(!done, warp_count, nullptr);     // (its barriers also publish `given`)
+        if (!done) { slot = given[rank]; done = true; }
+    }
+    if (t < batch && !with_replacement) claim[slot] = 0x7fffffff;   // leave the table clean
     if (t >= batch) return;
-    if (slot < 0) slot = below(rnd32(seed, step, t, draw++), (uint32_t)n_exist);  // (never in practice: 64 rounds)
     draw_or_zero<IdxT, kOwned>(indptr, indices, exist, slot, slot_lo, slot_hi, row0, n_items, seed, step, t, draw, users, pos, neg);
 }
 

@@ -27,6 +27,9 @@ class DeviceTripleSampler:
         csr = train_csr.tocsr()
         csr.sort_indices()
         self.n_users, self.n_items = csr.shape
+        full = np.nonzero(np.diff(csr.indptr) >= self.n_items)[0]
+        if len(full):
+            raise ValueError(f"user {int(full[0])} has every item in its training row: no negative item to draw")
         self.indptr = torch.from_numpy(csr.indptr.astype(np.int64)).to(device)
         self.indices = torch.from_numpy(csr.indices.astype(np.int64)).to(device)
         exist = np.nonzero(np.diff(csr.indptr) > 0)[0].astype(np.int64)
@@ -97,12 +100,17 @@ class ShardedTripleSampler:
         self.indices = dev(rows.indices, torch.int32)
         self.exist = torch.nonzero(self.indptr[1:] > self.indptr[:-1]).flatten()      # local rows, ascending
         n_local = self.exist.numel()
-        counts = [n_local] * part_u.world
-        if part_u.world > 1:
-            mine = torch.tensor([n_local], dtype=torch.int64, device=device)
+        full = torch.nonzero(self.indptr[1:] - self.indptr[:-1] >= self.n_items).flatten()
+        full_user = lo + int(full[0]) if full.numel() else -1       # a row holding every item: no negative to draw
+        counts, fulls = [n_local] * part_u.world, [full_user]
+        if part_u.world > 1:        # the full-row flag rides along, so every rank raises together and none waits in a collective
+            mine = torch.tensor([n_local, full_user], dtype=torch.int64, device=device)
             got = [torch.zeros_like(mine) for _ in range(part_u.world)]
             dist.all_gather(got, mine, group=group)
-            counts = [int(t.cpu()[0]) for t in got]
+            counts, fulls = [int(t.cpu()[0]) for t in got], [int(t.cpu()[1]) for t in got]
+        full_users = [u for u in fulls if u >= 0]
+        if full_users:
+            raise ValueError(f"user {full_users[0]} has every item in its training row: no negative item to draw")
         self.n_exist = sum(counts)
         if self.n_exist == 0:
             raise ValueError("no user has a training item")

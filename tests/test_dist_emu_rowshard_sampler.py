@@ -96,6 +96,8 @@ def _batches_worker(rank, world, port, ret):
                     got = mine.sample_into(torch.full((3, b), -1, dtype=torch.int64), step_dev=step_dev, step=0 if step_dev is not None else step)
                     if not torch.equal(got, want):
                         errs.append(f"{name}: B={b} step={step}: {(got != want).sum().item()} entries differ")
+                    if b <= mine.n_exist and len(torch.unique(got[0])) != b:
+                        errs.append(f"{name}: B={b} step={step}: {b - len(torch.unique(got[0]))} repeated users")
         ret[rank] = errs
     finally:
         dist.destroy_process_group()
