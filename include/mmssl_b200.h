@@ -369,6 +369,28 @@ int64_t mmssl_recommend_workspace_bytes(int64_t n, int k, int64_t n_items, int d
 int mmssl_recommend_topk(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
                          const int64_t* users, int64_t n, const int64_t* excl_indptr, const int64_t* excl_indices, int k,
                          int64_t ldo, int32_t* ids, float* scores, uint64_t* key_ws, void* stream);
+/* Sliced sweep: mmssl_recommend_topk with the candidates [0, n_items) cut into `slices` contiguous slices, slice s =
+ * [n_items * s / slices, n_items * (s + 1) / slices) (empty when slices > n_items), and every query ranked against every slice in
+ * one launch.  ids / scores [slices, n, k] (both required): row (s, i) is the best k of slice s for users[i], best first, with
+ * global candidate ids and the keys, ties and exclusion of the unsliced sweep, -1 / 0 past the end of a short list.  Merging the
+ * slices' lists of a row (mmssl_topk_merge, n_lists = slices) gives mmssl_recommend_topk's list bit for bit.  slices in
+ * 1..65535; key_ws must hold mmssl_recommend_sliced_workspace_bytes(n, k, n_items, d, slices) bytes (0 for k <= 64; with
+ * slices == 1 the bytes of mmssl_recommend_workspace_bytes). */
+int64_t mmssl_recommend_sliced_workspace_bytes(int64_t n, int k, int64_t n_items, int d, int slices);
+int mmssl_recommend_topk_sliced(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
+                                const int64_t* users, int64_t n, const int64_t* excl_indptr, const int64_t* excl_indices, int k,
+                                int slices, int32_t* ids, float* scores, uint64_t* key_ws, void* stream);
+/* Merge of partial top-k lists: for each of n rows, n_lists >= 1 lists of k entries, entry i of list q of row r at
+ * [q * list_stride + r * ld + i] (ld >= k), each list sorted best first by the sweep's key (higher score by the order-preserving
+ * transform of its fp32 bits, so -0.0 below +0.0; equal bits: lower id first) with -1 past its end, and no (score, id) in two
+ * lists of a row.  out_ids / out_scores [n, ldo] (ldo >= k) get the best k of the union, score bits copied, -1 / 0 past its end
+ * when it holds fewer than k.  One thread per entry counts the entries of the other lists that beat it (no atomics), so the result
+ * does not depend on the order of the lists.  Serves the slices of mmssl_recommend_topk_sliced and the ranks of a row-sharded
+ * model. */
+int mmssl_topk_merge(const int32_t* ids, const float* scores, int64_t n, int n_lists, int k, int64_t ld, int64_t list_stride,
+                     int32_t* out_ids, float* out_scores, int64_t ldo, void* stream);
+/* Streaming multiprocessors of the current device (0 if it cannot be queried): what a caller sizes a sliced launch by. */
+int mmssl_sm_count(void);
 
 /* ------------------------------------------------------------------ GAN side (SURVEY 8f "next" #2), see csrc/gan.cu
  * Device ops sequenced by mmssl_b200/gan.py; the Discriminator of Models.py:224-245 on n rows (LeakyReLU(True) is the

@@ -184,4 +184,17 @@ __device__ __forceinline__ float block_sum(float v, float* smem32) {
     return v;
 }
 
+// The ranking key of the top-k lists (eval.cu: the sweep and the merge of partial lists).  Larger key == better: higher score
+// first, then lower id.  fp32 -> order-preserving u32 of its bits, so -0.0 orders below +0.0 exactly as the sweep orders them.
+__device__ __forceinline__ uint64_t eval_key(float s, uint32_t item) {
+    uint32_t b = __float_as_uint(s);
+    b = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+    return ((uint64_t)b << 32) | (uint64_t)(0xFFFFFFFFu - item);
+}
+__device__ __forceinline__ float eval_key_score(uint64_t key) {
+    uint32_t b = (uint32_t)(key >> 32);
+    b = (b & 0x80000000u) ? (b & 0x7FFFFFFFu) : ~b;
+    return __uint_as_float(b);
+}
+
 }  // namespace mmssl

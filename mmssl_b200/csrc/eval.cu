@@ -32,6 +32,11 @@
 // Recommendation (mmssl_recommend_topk) is the kRec instantiation of both kernels: the same tile, sweep, buffers, compaction
 // and keys against an exclusion CSR in place of the training rows, one k, no held-out rows, no hits and no metrics; the best k
 // of each user go to ids / scores rows of leading dimension ldo.
+//
+// A few queries fill a few CTAs (8 per CTA), each sweeping every candidate.  mmssl_recommend_topk_sliced cuts the candidates
+// into contiguous slices and ranks every query tile against every slice in one launch (grid.y = slice), into partial lists with
+// global ids; mmssl_topk_merge merges the sorted partial lists of a row by the same unique keys, so the result is the unsliced
+// list bit for bit whatever the cut.  The same merge combines the partial lists of the ranks of a row-sharded model.
 #include "common.cuh"
 #include "../../include/mmssl_b200.h"
 
@@ -45,6 +50,7 @@ constexpr int kEvalCap = 512;      // candidate keys per user
 constexpr int kEvalMaxK = 64;      // max(Ks)
 constexpr int kEvalMaxKs = 8;
 constexpr int kEvalWideMaxK = 1 << 26;  // wide path: any K up to this (buffer offsets stay int)
+constexpr int kMaxSlices = 65535;       // slices of a sliced recommendation launch (gridDim.y)
 
 struct EvalKs {
     int n;
@@ -52,17 +58,7 @@ struct EvalKs {
     int k[kEvalMaxKs];
 };
 
-// Larger key == better: higher score first, then lower item id.  fp32 -> order-preserving u32.
-__device__ __forceinline__ uint64_t eval_key(float s, uint32_t item) {
-    uint32_t b = __float_as_uint(s);
-    b = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-    return ((uint64_t)b << 32) | (uint64_t)(0xFFFFFFFFu - item);
-}
-__device__ __forceinline__ float eval_key_score(uint64_t key) {
-    uint32_t b = (uint32_t)(key >> 32);
-    b = (b & 0x80000000u) ? (b & 0x7FFFFFFFu) : ~b;
-    return __uint_as_float(b);
-}
+// Keys: eval_key / eval_key_score (common.cuh), shared with the merge of partial lists (eval_merge_kernel).
 
 __device__ __forceinline__ bool row_contains(const int64_t* __restrict__ idx, int64_t lo, int64_t hi, int64_t x) {
     const int64_t end = hi;
@@ -262,12 +258,12 @@ __device__ __forceinline__ void eval_positives(EvalTile& t, uint32_t (*pstage)[k
     }
 }
 
-// One 128-item sweep from item `base`: in full mode the membership masks first (thread u walks user u's training row,
+// One 128-item sweep over the items [base, min(base + 128, end)): in full mode the membership masks first (thread u walks user u's training row,
 // thread 8 + u its held-out row, both sorted, so every id is visited once over the whole sweep), then every thread scores
 // its item against the 8 users, skips training items, counts the AUC pairs of negatives into `pairs` (full mode) and appends
 // every key that beats the user's threshold to the user's buffer keys[u * cap, ...).  Ends without a barrier.
 template <bool kFull>
-__device__ __forceinline__ void eval_sweep(EvalTile& t, int64_t base, const float* uvec, const float* __restrict__ item_emb,
+__device__ __forceinline__ void eval_sweep(EvalTile& t, int64_t base, int64_t end, const float* uvec, const float* __restrict__ item_emb,
                                            int64_t ldi, int64_t n_items, int d, const int64_t* __restrict__ tr_idx,
                                            const int64_t* __restrict__ he_ptr, const int64_t* __restrict__ he_idx,
                                            float* __restrict__ scores_out, int64_t tile0,
@@ -301,7 +297,7 @@ __device__ __forceinline__ void eval_sweep(EvalTile& t, int64_t base, const floa
         __syncthreads();
     }
     const int64_t j = base + tid;
-    if (j < n_items) {
+    if (j < end) {
         float acc[kEvalUsers];
         eval_dot<kEvalUsers>(item_emb + j * ldi, uvec, d, acc);
 #pragma unroll
@@ -356,8 +352,16 @@ __device__ __forceinline__ void eval_auc_finish(EvalTile& t, unsigned long long 
     }
 }
 
+// Slice blockIdx.y of gridDim.y contiguous slices of the candidates [0, n): [lo, hi), balanced to within one candidate, empty
+// when gridDim.y > n.  An unsliced launch (gridDim.y == 1) sweeps [0, n).
+__device__ __forceinline__ void eval_slice(int64_t n, int64_t& lo, int64_t& hi) {
+    lo = n * (int64_t)blockIdx.y / (int64_t)gridDim.y;
+    hi = n * ((int64_t)blockIdx.y + 1) / (int64_t)gridDim.y;
+}
+
 // kRec (recommendation): tr_* is the exclusion CSR, he_* / hits_out / per_user are unused, ks holds the one k, and ranked /
-// ranked_scores are rows of leading dimension ldo.
+// ranked_scores are rows of leading dimension ldo.  A sliced launch (gridDim.y > 1) ranks the candidates of slice
+// blockIdx.y (eval_slice; ids stay global) into rows blockIdx.y * n_eval + g of the output.
 template <bool kFull, bool kRec = false>
 __global__ void __launch_bounds__(kEvalThreads, kFull ? 2 : 0) eval_rank_kernel(
     const float* __restrict__ user_emb, int64_t ldu, const float* __restrict__ item_emb, int64_t ldi, int64_t n_items, int d,
@@ -383,8 +387,10 @@ __global__ void __launch_bounds__(kEvalThreads, kFull ? 2 : 0) eval_rank_kernel(
     unsigned long long pairs[kFull ? kEvalUsers : 1];                   // this thread's share of t.num[]
 #pragma unroll
     for (int u = 0; u < (kFull ? kEvalUsers : 1); ++u) pairs[u] = 0ull;
-    for (int64_t base = 0; base < n_items; base += kEvalThreads) {
-        eval_sweep<kFull>(t, base, uvec, item_emb, ldi, n_items, d, tr_idx, he_ptr, he_idx, scores_out, tile0, pairs, keys[0],
+    int64_t lo = 0, hi = n_items;
+    if constexpr (kRec) eval_slice(n_items, lo, hi);
+    for (int64_t base = lo; base < hi; base += kEvalThreads) {
+        eval_sweep<kFull>(t, base, hi, uvec, item_emb, ldi, n_items, d, tr_idx, he_ptr, he_idx, scores_out, tile0, pairs, keys[0],
                           kEvalCap, tid);
         __syncthreads();
         const int need = __syncthreads_or(tid < kEvalUsers && t.cnt[tid] > kEvalCap - kEvalThreads);
@@ -402,7 +408,8 @@ __global__ void __launch_bounds__(kEvalThreads, kFull ? 2 : 0) eval_rank_kernel(
         const int64_t g = tile0 + u;
         const int m = min(t.cnt[u], ks.kmax);                            // length of the hit list (batch_test.py:29-34)
         if constexpr (kRec) {                                            // the ranked list is the whole output
-            eval_write_list(keys[u], m, ks.kmax, ranked + g * ldo, ranked_scores ? ranked_scores + g * ldo : nullptr, lane);
+            const int64_t row = (int64_t)blockIdx.y * n_eval + g;
+            eval_write_list(keys[u], m, ks.kmax, ranked + row * ldo, ranked_scores ? ranked_scores + row * ldo : nullptr, lane);
             continue;
         }
         const int64_t hb = he_ptr[t.uid[u]], he = he_ptr[t.uid[u] + 1];
@@ -603,7 +610,7 @@ __global__ void __launch_bounds__(kEvalThreads, 1) eval_wide_kernel(
     extern __shared__ __align__(16) unsigned char eval_smem[];
     float* uvec = reinterpret_cast<float*>(eval_smem);
     // candidate buffers: after the user vectors (8 d floats, a multiple of 16 bytes), or the CTA's workspace slot
-    uint64_t* const keys = key_ws ? key_ws + (size_t)blockIdx.x * kEvalUsers * cap
+    uint64_t* const keys = key_ws ? key_ws + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * kEvalUsers * cap
                                   : reinterpret_cast<uint64_t*>(eval_smem + sizeof(float) * kEvalUsers * (size_t)d);
     __shared__ EvalTile t;
     __shared__ EvalRadix r;
@@ -623,8 +630,10 @@ __global__ void __launch_bounds__(kEvalThreads, 1) eval_wide_kernel(
         unsigned long long pairs[kFull ? kEvalUsers : 1];
 #pragma unroll
         for (int u = 0; u < (kFull ? kEvalUsers : 1); ++u) pairs[u] = 0ull;
-        for (int64_t base = 0; base < n_items; base += kEvalThreads) {
-            eval_sweep<kFull>(t, base, uvec, item_emb, ldi, n_items, d, tr_idx, he_ptr, he_idx, scores_out, tile0, pairs, keys, cap,
+        int64_t lo = 0, hi = n_items;
+        if constexpr (kRec) eval_slice(n_items, lo, hi);
+        for (int64_t base = lo; base < hi; base += kEvalThreads) {
+            eval_sweep<kFull>(t, base, hi, uvec, item_emb, ldi, n_items, d, tr_idx, he_ptr, he_idx, scores_out, tile0, pairs, keys, cap,
                               tid);
             __syncthreads();
             if (__syncthreads_or(tid < kEvalUsers && t.cnt[tid] > cap - kEvalThreads)) {
@@ -660,7 +669,8 @@ __global__ void __launch_bounds__(kEvalThreads, 1) eval_wide_kernel(
             const int m = t.cnt[u];                                      // length of the hit list (batch_test.py:29-34)
             const uint64_t* sk = sorted[u];
             if constexpr (kRec) {                                        // the ranked list is the whole output
-                eval_write_list(sk, m, kmax, ranked + g * ldo, ranked_scores ? ranked_scores + g * ldo : nullptr, lane);
+                const int64_t row = (int64_t)blockIdx.y * n_eval + g;
+                eval_write_list(sk, m, kmax, ranked + row * ldo, ranked_scores ? ranked_scores + row * ldo : nullptr, lane);
                 continue;
             }
             uint8_t* hitf = reinterpret_cast<uint8_t*>(sk == keys + (size_t)u * cap ? keys + (size_t)u * cap + ksel : keys + (size_t)u * cap);
@@ -743,6 +753,73 @@ __global__ void __launch_bounds__(256) eval_reduce_kernel(const double* __restri
     if (tid == 0) result[m] = n > 0 ? sh[0] / (double)n : 0.0;
 }
 
+// ---- merge of partial top-k lists (mmssl_topk_merge).  Element (r, q, i) is position i of list q of row r; a list holds its
+// entries best first and -1 past its end (a key of 0, below every real key).
+constexpr int kMergeThreads = 256;
+
+struct MergeLists {
+    const int32_t* ids;
+    const float* scores;
+    int64_t ld, stride;    // row r of list q starts at q * stride + r * ld
+    int k;
+    __device__ __forceinline__ uint64_t key(int64_t at) const {
+        const int32_t id = __ldg(ids + at);
+        return id < 0 ? 0ull : eval_key(__ldg(scores + at), (uint32_t)id);
+    }
+    // Entries of the list at `at` whose key beats x (x > 0): the length of its prefix of keys > x.
+    __device__ __forceinline__ int beating(int64_t at, uint64_t x) const {
+        if (key(at) <= x) return 0;                                      // the usual case for a key that makes the merged list
+        int lo = 1, hi = k;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (key(at + mid) > x) lo = mid + 1; else hi = mid;
+        }
+        return lo;
+    }
+    __device__ __forceinline__ int length(int64_t at) const {           // entries before the first -1
+        int lo = 0, hi = k;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (__ldg(ids + at + mid) >= 0) lo = mid + 1; else hi = mid;
+        }
+        return lo;
+    }
+};
+
+// One thread per element.  A real entry's place in the merged list is its position in its own list plus the entries of every
+// other list that beat it; keys are unique, so the places are distinct, and the sum does not depend on the lists' order.  It is
+// written (ids and score bits as they are) when the place is < k; the count stops as soon as it reaches k.  The threads of list
+// 0 also write -1 / 0 at position i when the lists hold at most i entries in all: those positions get no entry.
+__global__ void __launch_bounds__(kMergeThreads) eval_merge_kernel(MergeLists L, int64_t n, int P, int32_t* __restrict__ out_ids,
+                                                                   float* __restrict__ out_scores, int64_t ldo) {
+    const int64_t e = (int64_t)blockIdx.x * kMergeThreads + threadIdx.x;
+    const int64_t per_row = (int64_t)P * L.k;
+    if (e >= n * per_row) return;
+    const int64_t r = e / per_row;
+    const int q = (int)((e - r * per_row) / L.k), i = (int)(e - r * per_row - (int64_t)q * L.k);
+    const int64_t row = r * L.ld, at = (int64_t)q * L.stride + row + i;
+    const int32_t id = __ldg(L.ids + at);
+    if (id >= 0) {
+        const float sc = __ldg(L.scores + at);
+        const uint64_t x = eval_key(sc, (uint32_t)id);
+        int64_t place = i;
+        for (int q2 = 0; q2 < P && place < L.k; ++q2)
+            if (q2 != q) place += L.beating((int64_t)q2 * L.stride + row, x);
+        if (place < L.k) {
+            out_ids[r * ldo + place] = id;
+            out_scores[r * ldo + place] = sc;
+        }
+    }
+    if (q == 0) {
+        int64_t total = 0;
+        for (int q2 = 0; q2 < P && total <= i; ++q2) total += L.length((int64_t)q2 * L.stride + row);
+        if (total <= i) {
+            out_ids[r * ldo + i] = -1;
+            out_scores[r * ldo + i] = 0.f;
+        }
+    }
+}
+
 }  // namespace mmssl
 
 using namespace mmssl;
@@ -814,9 +891,10 @@ struct EvalWidePlan {
     int64_t grid, ws_keys;
 };
 
-static EvalWidePlan eval_wide_plan(int64_t n_eval, int kmax, int64_t n_items, int d) {
+static EvalWidePlan eval_wide_plan(int64_t n_eval, int kmax, int64_t n_items, int d, int slices = 1) {
     EvalWidePlan p;
-    p.ksel = (int)(kmax < n_items ? kmax : (n_items > 0 ? n_items : 1));
+    const int64_t span = (n_items + slices - 1) / slices;                // the longest slice's candidates
+    p.ksel = (int)(kmax < span ? kmax : (span > 0 ? span : 1));
     p.cap = (2 * p.ksel + 256 + 127) / 128 * 128;
     const int64_t n_tiles = (n_eval + kEvalUsers - 1) / kEvalUsers;
     const size_t slot = sizeof(uint64_t) * kEvalUsers * (size_t)p.cap;
@@ -828,9 +906,10 @@ static EvalWidePlan eval_wide_plan(int64_t n_eval, int kmax, int64_t n_items, in
     } else {
         int64_t slots = kEvalWideWsBytes / (int64_t)slot;
         slots = slots < 1 ? 1 : (slots > kEvalWideSlots ? kEvalWideSlots : slots);
+        const int64_t per_slice = slots / slices > 1 ? slots / slices : 1;   // a sliced launch: grid x slices CTAs, one slot each
         p.smem = uvec;
-        p.grid = n_tiles < slots ? n_tiles : slots;
-        p.ws_keys = p.grid * kEvalUsers * (int64_t)p.cap;
+        p.grid = n_tiles < per_slice ? n_tiles : per_slice;
+        p.ws_keys = p.grid * slices * kEvalUsers * (int64_t)p.cap;
     }
     return p;
 }
@@ -885,14 +964,15 @@ extern "C" int64_t mmssl_recommend_workspace_bytes(int64_t n, int k, int64_t n_i
     return k <= kEvalMaxK ? 0 : mmssl_eval_wide_workspace_bytes(n, k, n_items, d);
 }
 
-extern "C" int mmssl_recommend_topk(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
-                                    const int64_t* users, int64_t n, const int64_t* excl_indptr, const int64_t* excl_indices, int k,
-                                    int64_t ldo, int32_t* ids, float* scores, uint64_t* key_ws, void* stream_) {
+static int recommend_launch(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
+                            const int64_t* users, int64_t n, const int64_t* excl_indptr, const int64_t* excl_indices, int k,
+                            int slices, int64_t ldo, int32_t* ids, float* scores, uint64_t* key_ws, void* stream_) {
     MMSSL_REQUIRE(d >= 4 && d <= 256 && (d & 3) == 0, "embedding width must be a multiple of 4, at most 256");
     MMSSL_REQUIRE((ldi & 3) == 0 && aligned16(item_emb), "item table rows must be 16-byte aligned");
     MMSSL_REQUIRE(n_items >= 0 && n_items < (1ll << 31), "bad item count");
     MMSSL_REQUIRE(k >= 1 && k <= kEvalWideMaxK, "k must be in 1..2^26");
     MMSSL_REQUIRE(ldo >= k, "ldo must be at least k");
+    MMSSL_REQUIRE(slices >= 1 && slices <= kMaxSlices, "slices must be in 1..65535");
     MMSSL_REQUIRE(ids != nullptr && excl_indptr != nullptr && excl_indices != nullptr, "ids and the exclusion CSR are required");
     if (n == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream_;
@@ -903,20 +983,66 @@ extern "C" int mmssl_recommend_topk(const float* user_emb, int64_t ldu, const fl
         for (int q = 0; q < kEvalMaxKs; ++q) ks.k[q] = 0;
         ks.k[0] = k;
         const size_t smem = sizeof(uint64_t) * kEvalUsers * kEvalCap + sizeof(float) * kEvalUsers * (size_t)d;
-        const unsigned grid = (unsigned)((n + kEvalUsers - 1) / kEvalUsers);
+        const dim3 grid((unsigned)((n + kEvalUsers - 1) / kEvalUsers), (unsigned)slices);
         eval_rank_kernel<false, true><<<grid, kEvalThreads, smem, st>>>(
             user_emb, ldu, item_emb, ldi, n_items, d, users, n, excl_indptr, excl_indices, nullptr, nullptr, ks, ids, scores, nullptr,
             nullptr, nullptr, nullptr, nullptr, nullptr, ldo);
     } else {
-        const EvalWidePlan p = eval_wide_plan(n, k, n_items, d);
+        const EvalWidePlan p = eval_wide_plan(n, k, n_items, d, slices);
         MMSSL_REQUIRE(p.ws_keys == 0 || key_ws != nullptr, "key_ws (mmssl_recommend_workspace_bytes) is required");
         MMSSL_CUDA(cudaFuncSetAttribute(eval_wide_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-        eval_wide_kernel<false, true><<<(unsigned)p.grid, kEvalThreads, p.smem, st>>>(
+        eval_wide_kernel<false, true><<<dim3((unsigned)p.grid, (unsigned)slices), kEvalThreads, p.smem, st>>>(
             user_emb, ldu, item_emb, ldi, n_items, d, users, n, excl_indptr, excl_indices, nullptr, nullptr, nullptr, 0, k, p.ksel,
             p.cap, p.ws_keys ? key_ws : nullptr, ids, scores, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, ldo);
     }
     MMSSL_LAUNCH_OK();
     return 0;
+}
+
+extern "C" int mmssl_recommend_topk(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items, int d,
+                                    const int64_t* users, int64_t n, const int64_t* excl_indptr, const int64_t* excl_indices, int k,
+                                    int64_t ldo, int32_t* ids, float* scores, uint64_t* key_ws, void* stream_) {
+    return recommend_launch(user_emb, ldu, item_emb, ldi, n_items, d, users, n, excl_indptr, excl_indices, k, 1, ldo, ids, scores,
+                            key_ws, stream_);
+}
+
+// Sliced sweep: the candidates [0, n_items) in `slices` contiguous slices (eval_slice), every query against every slice in one
+// launch of grid (query tiles, slices), partial lists [slices, n, k].  Same routes, kernels, dot product, keys and exclusion
+// search as mmssl_recommend_topk, with global candidate ids, so merging the partial lists (mmssl_topk_merge) gives its lists.
+extern "C" int64_t mmssl_recommend_sliced_workspace_bytes(int64_t n, int k, int64_t n_items, int d, int slices) {
+    if (n <= 0 || k <= kEvalMaxK || k > kEvalWideMaxK || d < 4 || slices < 1 || slices > kMaxSlices) return 0;
+    return eval_wide_plan(n, k, n_items, d, slices).ws_keys * (int64_t)sizeof(uint64_t);
+}
+
+extern "C" int mmssl_recommend_topk_sliced(const float* user_emb, int64_t ldu, const float* item_emb, int64_t ldi, int64_t n_items,
+                                           int d, const int64_t* users, int64_t n, const int64_t* excl_indptr,
+                                           const int64_t* excl_indices, int k, int slices, int32_t* ids, float* scores,
+                                           uint64_t* key_ws, void* stream_) {
+    MMSSL_REQUIRE(scores != nullptr, "the partial lists' scores are required (the merge orders by them)");
+    return recommend_launch(user_emb, ldu, item_emb, ldi, n_items, d, users, n, excl_indptr, excl_indices, k, slices, k, ids, scores,
+                            key_ws, stream_);
+}
+
+extern "C" int mmssl_topk_merge(const int32_t* ids, const float* scores, int64_t n, int n_lists, int k, int64_t ld,
+                                int64_t list_stride, int32_t* out_ids, float* out_scores, int64_t ldo, void* stream_) {
+    MMSSL_REQUIRE(n >= 0 && n_lists >= 1 && k >= 1 && k <= kEvalWideMaxK, "n >= 0, n_lists >= 1 and k in 1..2^26");
+    MMSSL_REQUIRE(ld >= k && ldo >= k && list_stride >= 0, "ld and ldo must be at least k, list_stride >= 0");
+    MMSSL_REQUIRE(ids != nullptr && scores != nullptr && out_ids != nullptr && out_scores != nullptr, "all four arrays are required");
+    const int64_t threads = n * (int64_t)n_lists * k;
+    if (threads == 0) return 0;
+    MergeLists L{ids, scores, ld, list_stride, k};
+    const int64_t grid = (threads + kMergeThreads - 1) / kMergeThreads;
+    MMSSL_REQUIRE(grid < (1ll << 31), "too many elements for one merge launch");
+    eval_merge_kernel<<<(unsigned)grid, kMergeThreads, 0, (cudaStream_t)stream_>>>(L, n, n_lists, out_ids, out_scores, ldo);
+    MMSSL_LAUNCH_OK();
+    return 0;
+}
+
+extern "C" int mmssl_sm_count(void) {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+        return 0;
+    return sms;
 }
 
 extern "C" int mmssl_eval_reduce(const double* per_user, int64_t n_eval, int n_metrics, double* result, void* stream_) {

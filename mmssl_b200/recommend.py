@@ -158,6 +158,22 @@ class _Files:
                 os.remove(p)
 
 
+# Slicing of the candidates (Recommender._slices)
+_SLICE_CTAS_PER_SM = 2              # CTAs per SM a launch should reach before it is left unsliced
+_SLICE_MIN = 4096                   # candidates per slice at least: a shorter slice costs more in setup and merge than it saves
+_SLICE_BYTES = 256 << 20            # device memory of the partial lists (ids and scores, slices x n x k) at most
+_MAX_SLICES = 65535
+
+
+def merge_lists(ids: torch.Tensor, scores: torch.Tensor, n: int, n_lists: int, k: int, ld: int, stride: int, out_ids: torch.Tensor,
+                out_scores: torch.Tensor, ldo: int) -> None:
+    """``mmssl_topk_merge``: the best k of n_lists sorted partial lists per row (entry i of list q of row r at element
+    q * stride + r * ld + i of ids / scores) into rows of leading dimension ldo of out_ids / out_scores."""
+    if n:
+        _lib.check(_lib.load().mmssl_topk_merge(ptr(ids), ptr(scores), n, n_lists, k, ld, stride, ptr(out_ids), ptr(out_scores), ldo,
+                                                stream()))
+
+
 def _check_sorted_rows(indptr: torch.Tensor, indices: torch.Tensor) -> None:
     """The kernel finds excluded items by binary search in each row: an unsorted row would let excluded items through."""
     nnz = indices.numel()
@@ -192,6 +208,7 @@ class Recommender:
         _check_sorted_rows(ip, ix)
         self.exclude, self.n_users = (ip, ix), ip.numel() - 1
         self.device = ia.device
+        self.sms = _lib.load().mmssl_sm_count()
 
     @classmethod
     def from_rows(cls, item_table: torch.Tensor, train_items, test_set, val_set, n_users: int, k: int,
@@ -213,15 +230,41 @@ class Recommender:
             raise ValueError(f"user table of width {ua.shape[-1]}, the item table's is {self.d}")
         return ua if ua.stride(1) == 1 else ua.contiguous()
 
-    def _launch(self, ua, users_dev, n: int, ids, scores, ldo: int, key_ws) -> None:
-        """Ranks users_dev[0, n) into ids / scores rows of leading dimension ldo (n > 0)."""
+    def _slices(self, n: int) -> int:
+        """How many contiguous slices of the candidates a launch of n queries ranks separately (1: the unsliced sweep).  The sweep
+        gives a CTA 8 queries and every candidate, so fewer than _SLICE_CTAS_PER_SM CTAs per SM leave SMs idle; slicing fills
+        them, as long as a slice keeps at least _SLICE_MIN (and 8 k) candidates and the partial lists stay within _SLICE_BYTES.
+        The merged lists are the unsliced lists bit for bit, so this choice changes the time of a call, never its result."""
+        if n < 1:
+            return 1
+        tiles = -(-n // 8)
+        want = -(-_SLICE_CTAS_PER_SM * self.sms // tiles)
+        most = self.n_items // max(_SLICE_MIN, 8 * self.k)
+        fits = _SLICE_BYTES // (8 * n * self.k)
+        return max(1, min(want, most, fits, _MAX_SLICES))
+
+    def _launch(self, ua, users_dev, n: int, ids, scores, ldo: int, key_ws=None) -> None:
+        """Ranks users_dev[0, n) into ids / scores rows of leading dimension ldo (n > 0): one sweep, or a sliced sweep into
+        partial lists and their merge (_slices).  key_ws: a workspace from _key_ws, replaced here when it is too small."""
         lib = _lib.load()
-        _lib.check(lib.mmssl_recommend_topk(ptr(ua), ua.stride(0), ptr(self.items), self.items.stride(0), self.n_items, self.d,
-                                            ptr(users_dev), n, ptr(self.exclude[0]), ptr(self.exclude[1]), self.k, ldo, ptr(ids),
-                                            ptr(scores), ptr(key_ws), stream()))
+        s = self._slices(n)
+        if key_ws is None or key_ws.numel() * 8 < self._ws_bytes(n, s):
+            key_ws = self._key_ws(n)
+        args = (ptr(ua), ua.stride(0), ptr(self.items), self.items.stride(0), self.n_items, self.d, ptr(users_dev), n,
+                ptr(self.exclude[0]), ptr(self.exclude[1]), self.k)
+        if s == 1:
+            _lib.check(lib.mmssl_recommend_topk(*args, ldo, ptr(ids), ptr(scores), ptr(key_ws), stream()))
+            return
+        part_ids = torch.empty(s, n, self.k, dtype=torch.int32, device=self.device)
+        part_sc = torch.empty(s, n, self.k, dtype=torch.float32, device=self.device)
+        _lib.check(lib.mmssl_recommend_topk_sliced(*args, s, ptr(part_ids), ptr(part_sc), ptr(key_ws), stream()))
+        merge_lists(part_ids, part_sc, n, s, self.k, self.k, n * self.k, ids, scores, ldo)
+
+    def _ws_bytes(self, n: int, s: int) -> int:
+        return _lib.load().mmssl_recommend_sliced_workspace_bytes(n, self.k, self.n_items, self.d, s)
 
     def _key_ws(self, n: int):
-        nbytes = _lib.load().mmssl_recommend_workspace_bytes(n, self.k, self.n_items, self.d)
+        nbytes = self._ws_bytes(n, self._slices(n))
         return torch.empty(nbytes // 8, dtype=torch.int64, device=self.device) if nbytes else None
 
     def topk(self, user_table: torch.Tensor, users) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -232,7 +275,7 @@ class Recommender:
         ids = torch.empty(n, self.k, dtype=torch.int32, device=dev)
         scores = torch.empty(n, self.k, dtype=torch.float32, device=dev)
         if n:
-            self._launch(ua, torch.from_numpy(ids_np).to(dev), n, ids, scores, self.k, self._key_ws(n))
+            self._launch(ua, torch.from_numpy(ids_np).to(dev), n, ids, scores, self.k)
         return ids.to(torch.int64), scores
 
     def export(self, user_table: torch.Tensor, users, out_dir: str, chunk: int = 1 << 16, prefix: str = "") -> int:
@@ -318,7 +361,8 @@ def _load_set(out_dir: str, prefix: str, meta: dict, query: str = "users"):
 
 # the readers of the export formats that share the file logic above: a directory of one kind is refused by the other's reader
 READERS = {FORMAT: "recommendations (mmssl_b200.recommend.read)",
-           "mmssl_b200.similar.v1": "similar items (mmssl_b200.similar.read)"}
+           "mmssl_b200.similar.v1": "similar items (mmssl_b200.similar.read)",
+           "mmssl_b200.audience.v1": "audiences (mmssl_b200.audience.read)"}
 
 
 def _check_format(out_dir: str, meta: dict, fmt: str) -> None:

@@ -201,6 +201,34 @@ class Trainer:
         rec, user_table = self.recommender(k, exclude)
         return rec.topk(user_table, users)
 
+    _audience_rows = None                             # exclusion set -> its transposed (item -> users) CSR, built on first use
+
+    def audience_ranker(self, k: int, exclude: str = "train"):
+        """(audience.Audience over the model's user table, the item table) of the eval-mode forward ``test`` and ``recommender``
+        run, excluding per item the users who had it in training ("train") or also in validation or test ("seen").
+        ``audience`` ranks with it; ``Audience.export`` writes the lists to files."""
+        from .audience import Audience, transpose_csr
+        from .dataset import held_csr
+        from .evaluate import _device_csr
+        from .recommend import EXCLUDE, exclusion_rows
+        if exclude not in EXCLUDE:
+            raise ValueError(f"exclude must be one of {EXCLUDE}, not {exclude!r}")
+        if self._audience_rows is None:
+            self._audience_rows = {}
+        if exclude not in self._audience_rows:
+            d = self.data
+            rows = held_csr(exclusion_rows(d.train_items, d.test_set, d.val_set, exclude), self.n_users)
+            self._audience_rows[exclude] = _device_csr(*transpose_csr(*rows, self.n_items), self.device)
+        hs = self.step.hs
+        outs, _ = hs.engine.forward(hs.P, hs.feats, hs.graphs, None, want_sumsq=False)       # model.eval(): no dropout
+        return Audience(outs[0], self._audience_rows[exclude], k), outs[1]
+
+    def audience(self, items, k: int, exclude: str = "train"):
+        """The k users each of `items` should be shown to: (ids [n, k] int64 user ids, scores [n, k] fp32) on the device, best
+        first, -1 past the end of a short list.  A score is the one ``recommend`` gives the same (user, item) pair (audience.py)."""
+        aud, item_table = self.audience_ranker(k, exclude)
+        return aud.topk(item_table, items)
+
     def similar(self, k: int, space: str = "model"):
         """similar.SimilarItems over the table of `space` of the eval-mode model ``test`` and ``recommender`` use: the final item
         table ("model", from the same forward, with the full step's current modality graphs) or a modality projection ("image",

@@ -11,7 +11,13 @@
     Neither checkpoint kind stores id_cat_rate / model_cat_rate, which shape the eval-mode forward: a run trained with other
     values than the defaults (0.36 / 0.55) needs --id-cat-rate / --model-cat-rate, in both modes.
 
-``recommend.read(DIR)`` returns (users, ids, scores) of either layout.  Prints one JSON line (rank 0)."""
+    --audience [--items FILE]: in either mode, export the audiences of items instead -- the top-k users of each item
+        (mmssl_b200/audience.py) -- as DIR/{ids,scores,items}.npy (or rankRRRRR-of-WWWWW.*, a rank writing the items of its item
+        block): of every item, or of the int64 item ids in FILE (.npy).  --exclude drops the users who had the item in training
+        ("train") or also in val / test ("seen"); --chunk then counts items.
+
+``recommend.read(DIR)`` returns (users, ids, scores) of either layout, ``audience.read(DIR)`` (items, ids, scores).  Prints one JSON
+line (rank 0)."""
 import argparse
 import json
 import os
@@ -24,10 +30,14 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
-from mmssl_b200 import checkpoint, recommend  # noqa: E402
+from mmssl_b200 import audience, checkpoint, recommend  # noqa: E402
 
 
-def one_gpu(a, dev):
+def _items(a, n_items: int) -> np.ndarray:
+    return np.load(a.items).astype(np.int64).reshape(-1) if a.items else np.arange(n_items, dtype=np.int64)
+
+
+def load_trainer(a, dev):
     from mmssl_b200.dataset import ReferenceDataset
     from mmssl_b200.trainer import Trainer, TrainerArgs
     st = checkpoint.load(a.checkpoint, kinds=("trainer",))
@@ -42,12 +52,22 @@ def one_gpu(a, dev):
     ds = ReferenceDataset.load(a.data)
     t = Trainer(ds, args, device=dev, sampler=tr["sampler"], log=None)
     t.load(a.checkpoint)
+    return t
+
+
+def one_gpu(a, dev):
+    t = load_trainer(a, dev)
+    if a.audience:
+        aud, item_table = t.audience_ranker(a.k, a.exclude)         # what Trainer.audience ranks with
+        n = aud.export(item_table, _items(a, t.n_items), a.out, chunk=a.chunk)
+        return dict(audiences=n, users=t.n_users, items=t.n_items)
     rec, user_table = t.recommender(a.k, a.exclude)                 # what Trainer.recommend ranks with
     n = rec.export(user_table, np.arange(t.n_users, dtype=np.int64), a.out, chunk=a.chunk)
     return dict(users=n, items=t.n_items)
 
 
-def sharded(a, dev, rank, world):
+def load_sharded(a, dev, rank, world):
+    """(the rank's ShardedDataset, its padded blocks of the final user and item tables) of the row-sharded checkpoint."""
     from mmssl_b200.dataset import ShardedDataset
     from mmssl_b200.engine import P_EI, P_EU
     from mmssl_b200.hotstep import HotStepConfig
@@ -70,6 +90,15 @@ def sharded(a, dev, rank, world):
     del st, P
     step.load(a.sharded)
     u_f, i_f = step.final_embeddings()
+    return sh, u_f, i_f
+
+
+def sharded(a, dev, rank, world):
+    sh, u_f, i_f = load_sharded(a, dev, rank, world)
+    if a.audience:
+        aud = audience.ShardedAudience.from_shards(sh, a.k, a.exclude, device=dev)
+        n = aud.export(u_f, i_f, _items(a, sh.n_items), a.out, chunk=a.chunk)
+        return dict(users=sh.n_users, items=sh.n_items, rows_written_by_rank0=n)
     rec = recommend.ShardedRecommender.from_shards(sh, a.k, a.exclude, device=dev)
     n = rec.export(u_f, i_f, np.arange(sh.n_users, dtype=np.int64), a.out, chunk=a.chunk)
     return dict(users=sh.n_users, items=sh.n_items, rows_written_by_rank0=n)
@@ -84,13 +113,17 @@ def main(argv=None):
     ap.add_argument("--k", type=int, default=20)
     ap.add_argument("--exclude", choices=recommend.EXCLUDE, default="train")
     ap.add_argument("--out", required=True)
-    ap.add_argument("--chunk", type=int, default=1 << 16, help="users ranked per launch (bounds the device memory)")
+    ap.add_argument("--chunk", type=int, default=1 << 16, help="users (items with --audience) ranked per launch (bounds the device memory)")
+    ap.add_argument("--audience", action="store_true", help="export the top-k users of items instead of the top-k items of users")
+    ap.add_argument("--items", help="with --audience: a .npy of the item ids to rank (default: every item)")
     # both rates shape the eval-mode forward and neither checkpoint kind stores them: give the trained run's values
     ap.add_argument("--id-cat-rate", type=float, default=0.36, help="the run's id_cat_rate (not in its checkpoint; default 0.36)")
     ap.add_argument("--model-cat-rate", type=float, default=0.55, help="the run's model_cat_rate (not in its checkpoint; default 0.55)")
     a = ap.parse_args(argv)
     if bool(a.sharded) == bool(a.checkpoint) or (a.sharded and not a.shards) or (a.checkpoint and not a.data):
         ap.error("give DATA --checkpoint FILE, or --sharded DIR --shards DIR")
+    if a.items and not a.audience:
+        ap.error("--items needs --audience")
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
