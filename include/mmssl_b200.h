@@ -192,6 +192,25 @@ int mmssl_softmax_bwd(const float* y, int64_t ldy, const float* g, int64_t ldg, 
 /* out = x / max(|x|_2, 1e-12) row by row (F.normalize; a zero row stays zero), strided [n, d] rows at the six embedding widths.
  * A row's result depends on that row only, not on n or the launch shape (the unit tables of item-to-item similarity). */
 int mmssl_unit_rows(const float* x, int64_t ldx, int64_t n, int d, float* out, int64_t ldo, void* stream);
+/* Fold-in (mmssl_b200/foldin.py): the final user row of each query -- an item list, with the item side of the model held fixed --
+ * by the closed form of the forward (SURVEY appendix A):
+ *   u_{k+1} = w * sum_{j in row} layer[k][j]  (k < K; row softmax over d on k = K-1),   Uv = w * sum Xv[j],   Ut = w * sum Xt[j],
+ *   out = (u_0 + u_1 + ... + u_K) * inv_layers + rate * (normalize(Uv) + normalize(Ut))
+ * u_0 = u0[users[q]] (users[q] >= 0) or 0 (-1, a user the model never trained on).  Each sum is formed as the SpMM forms a
+ * training row: a sequential fmaf chain in the row's order from +0.0f, and a row longer than the plan's split threshold cut into
+ * the plan's segments whose sums are added in segment order (also above the heavy threshold: no atomics); the softmax, running
+ * sum and combine are the forward's kernels' arithmetic.  Query q is indices[indptr[q], indptr[q+1]) (int64, sorted, distinct,
+ * in [0, n_items): the caller checks), w[q] its fp32 row weight.  A row's result depends on that row only.  n_layers in
+ * 0..MMSSL_FOLD_MAX_LAYERS; every table 16-byte aligned with ld % 4 == 0. */
+#define MMSSL_FOLD_MAX_LAYERS 6
+typedef struct {
+    const float* layer[MMSSL_FOLD_MAX_LAYERS]; int64_t ld_layer[MMSSL_FOLD_MAX_LAYERS];   /* i_0 .. i_{K-1} of the forward */
+    const float* xv; int64_t ldxv;                                                          /* the projections Xv, Xt */
+    const float* xt; int64_t ldxt;
+} mmssl_fold_tables_t;
+int mmssl_fold_users(const int64_t* indptr, const int64_t* indices, const int64_t* users, const float* w, int64_t n,
+                     const float* u0, int64_t ldu0, const mmssl_fold_tables_t* tables /*host*/, int d, int n_layers,
+                     float inv_layers, float rate, float* out, int64_t ldo, void* stream);
 /* y = alpha * (alpha_dev ? *alpha_dev : 1) * x + beta * y, strided rows (alpha_dev: optional device scalar) */
 int mmssl_axpby(const float* x, int64_t ldx, int64_t n, int d, float alpha, const float* alpha_dev, float beta, float* y, int64_t ldy, void* stream);
 /* dropout apply: y = x * mask (mask holds 0 or 1/(1-p)) ; mask may be NULL (copy) */

@@ -38,6 +38,15 @@ class SpmmRhs(C.Structure):
                 ("y_mode", C.c_int32), ("n_peers", C.c_int32), ("y_peers", c_vp * 8)]
 
 
+FOLD_MAX_LAYERS = 6                     # MMSSL_FOLD_MAX_LAYERS
+
+
+class FoldTables(C.Structure):
+    """mmssl_fold_tables_t"""
+    _fields_ = [("layer", c_vp * FOLD_MAX_LAYERS), ("ld_layer", c_i64 * FOLD_MAX_LAYERS), ("xv", c_vp), ("ldxv", c_i64),
+                ("xt", c_vp), ("ldxt", c_i64)]
+
+
 _SIGS = {
     "mmssl_abi_version": (C.c_int, []),
     "mmssl_last_error": (C.c_char_p, []),
@@ -80,6 +89,8 @@ _SIGS = {
                                     c_f32, c_f32, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "mmssl_softmax_bwd": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_f32, c_vp, c_i64, c_vp]),
     "mmssl_unit_rows": (C.c_int, [c_vp, c_i64, c_i64, c_i32, c_vp, c_i64, c_vp]),
+    "mmssl_fold_users": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, C.POINTER(FoldTables), c_i32, c_i32, c_f32, c_f32, c_vp,
+                                   c_i64, c_vp]),
     "mmssl_axpby": (C.c_int, [c_vp, c_i64, c_i64, c_i32, c_f32, c_vp, c_f32, c_vp, c_i64, c_vp]),
     "mmssl_mul_mask": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_i64, c_vp]),
     "mmssl_sumsq_blocks": (c_i64, [c_i64, c_i32]),
@@ -182,7 +193,7 @@ KERNELS_PER_CALL = {
     "mmssl_csr_from_coo": 6, "mmssl_csr_row_normalize": 1, "mmssl_spmm_plan": 8, "mmssl_spmm_csr_f32": 1, "mmssl_spmm_hot_f32": 1, "mmssl_spmm_bulk_plan": 9, "mmssl_spmm_bulk_f32": 1, "mmssl_reduce_rows_epilogue": 1, "mmssl_sgemm": 1,
     "mmssl_id_fuse_fwd": 1, "mmssl_id_fuse_bwd": 1, "mmssl_wsum": 1, "mmssl_id_fuse2_fwd": 1, "mmssl_id_fuse2_bwd": 1,
     "mmssl_dwcat_reduce": 1, "mmssl_combine_fwd": 1, "mmssl_combine_bwd": 1, "mmssl_softmax_bwd": 1,
-    "mmssl_unit_rows": 1, "mmssl_axpby": 1, "mmssl_mul_mask": 1, "mmssl_sumsq": 1, "mmssl_bpr": 1, "mmssl_infonce_prepare": 1,
+    "mmssl_unit_rows": 1, "mmssl_fold_users": 1, "mmssl_axpby": 1, "mmssl_mul_mask": 1, "mmssl_sumsq": 1, "mmssl_bpr": 1, "mmssl_infonce_prepare": 1,
     "mmssl_infonce_stats": 2, "mmssl_infonce_grad": 1, "mmssl_infonce_scatter": 1, "mmssl_infonce_stats_tc": 4, "mmssl_infonce_forward_tc": 3, "mmssl_infonce_grad_tc": 1, "mmssl_loss_assemble": 1,
     "mmssl_step_tick": 1, "mmssl_dp_fused_adamw": 1, "mmssl_dp_fused_adamw_dev": 1, "mmssl_sampler_init": 1, "mmssl_sample_triples": 1, "mmssl_sample_triples_multi": 20, "mmssl_sample_triples_owned": 1, "mmssl_sample_triples_multi_owned": 20, "mmssl_adamw": 1, "mmssl_split_bf16": 1, "mmssl_split_bf16_t": 1, "mmssl_split_bf16_t_colsum": 1, "mmssl_gemm_bf16x3": 1, "mmssl_gemm_bf16x3_group": 1, "mmssl_gemm_bf16x3_wide": 1,
     "mmssl_proj_epilogue": 1, "mmssl_wgrad_epilogue": 1, "mmssl_colsum": 1,

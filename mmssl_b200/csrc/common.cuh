@@ -160,6 +160,10 @@ constexpr WidthShape width_shape(int d) {
 constexpr bool width_supported(int d) { return width_shape(d).g != 0; }
 int fail_width(const char* where, int d);   // "<where>: embedding width <d> is not supported (...)"
 
+// The SpMM work plan's current row cuts (graph.cu, mmssl_spmm_plan_set_cuts): {split threshold, segment length, heavy threshold,
+// heavy segment length}.  The fold-in kernel (rowops.cu) cuts a query row where the plan would cut a training row.
+int4 spmm_plan_cuts();
+
 // f(integral_constant G, integral_constant C) for one of the six widths, an error naming the width otherwise.
 template <typename F>
 static inline int dispatch_width(int d, F&& f, const char* where = "embedding width") {

@@ -96,6 +96,7 @@ static cudaError_t carve_csr_ws(int64_t nnz, int64_t n_rows, void* base, CsrWs* 
 struct PlanCuts { int split_threshold, seg_len, heavy_threshold, heavy_seg_len; };
 static PlanCuts g_cuts = {64, 32, 1024, 64};
 __host__ __device__ __forceinline__ int plan_seg_len(int len, const PlanCuts c) { return len <= c.heavy_threshold ? c.seg_len : c.heavy_seg_len; }
+int4 spmm_plan_cuts() { return make_int4(g_cuts.split_threshold, g_cuts.seg_len, g_cuts.heavy_threshold, g_cuts.heavy_seg_len); }
 
 __global__ void plan_count_kernel(const int32_t* __restrict__ rowptr, int64_t n_rows,
                                   int32_t* __restrict__ n_items, int32_t* __restrict__ is_split,

@@ -6,6 +6,7 @@
 //                                    (+ the sums of squares main.py:252-257 needs, for free)
 //   softmax_bwd  backward of Models.py:203-204
 //   unit_rows    out = normalize(x): the unit tables of item-to-item similarity (similar.py)
+//   fold_users   the final user row of an item list with the item side held fixed (foldin.py): gathers + the combine above
 #include "common.cuh"
 #include "../../include/mmssl_b200.h"
 
@@ -226,6 +227,162 @@ __global__ void __launch_bounds__(256) unit_rows_kernel(const float* __restrict_
     store_row<G, C>(v, out, ldo, ix);
 }
 
+// ---- fold-in: the final user row of an item list, the item side held fixed (foldin.py) ----
+// A CTA holds Q queries and (K+2) lane groups per query, one per table: layer k (k < K) sums i_k into u_{k+1}, group K sums Xv
+// into Uv, group K+1 Xt into Ut.  The per-table rows meet in shared memory and the query's first group combines them.  Every sum
+// repeats spmm_item's arithmetic for an R-right-hand-side launch (R = 1 for the layers, 2 for the image|text pair): chunks of G
+// (col, val) pairs, UNR gathers per round with zero-padded FMAs past the end, and for a split row the segment sums added from
+// +0.0f in segment order, PB at a time with zero padding.  Those padded operations only turn a -0.0 sum into +0.0, as they do
+// in the SpMM.
+template <int G, int C, int R>
+__device__ __forceinline__ void fold_walk(float4 (&acc)[C], const int64_t* __restrict__ idx, int64_t b, int64_t e, float w,
+                                          const float* __restrict__ x, int64_t ldx, int lane, unsigned mask) {
+    constexpr int UNR0 = (8 / (R * C)) >= 2 ? (8 / (R * C)) : 2;
+    constexpr int UNR = UNR0 > G ? G : UNR0;
+#pragma unroll
+    for (int c = 0; c < C; ++c) acc[c] = f4zero();
+    for (int64_t base = b; base < e; base += G) {
+        const long long my = (base + lane < e) ? (long long)__ldg(reinterpret_cast<const long long*>(idx) + base + lane) : 0ll;
+        const float v_l = (base + lane < e) ? w : 0.f;
+        const int cnt = (int)((e - base) < G ? (e - base) : G);
+        for (int j = 0; j < cnt; j += UNR) {
+            long long cc[UNR];
+            float vv[UNR];
+#pragma unroll
+            for (int k = 0; k < UNR; ++k) {
+                cc[k] = __shfl_sync(mask, my, j + k, G);
+                vv[k] = __shfl_sync(mask, v_l, j + k, G);
+            }
+            float4 xv[UNR][C];
+#pragma unroll
+            for (int k = 0; k < UNR; ++k) {
+                const bool on = (j + k) < cnt;
+                const float* xr = x + (int64_t)cc[k] * ldx + lane * 4;
+#pragma unroll
+                for (int c = 0; c < C; ++c) xv[k][c] = on ? ldg4(xr + c * (4 * G)) : f4zero();
+            }
+#pragma unroll
+            for (int k = 0; k < UNR; ++k)
+#pragma unroll
+                for (int c = 0; c < C; ++c) fma4(acc[c], vv[k], xv[k][c]);
+        }
+    }
+}
+
+template <int G, int C, int R>
+__device__ __forceinline__ void fold_sum(float4 (&acc)[C], const int64_t* __restrict__ idx, int64_t b, int64_t e, float w,
+                                         const float* __restrict__ x, int64_t ldx, const int4 cuts, int lane, unsigned mask) {
+    const int64_t len = e - b;
+    if (len <= cuts.x) {
+        fold_walk<G, C, R>(acc, idx, b, e, w, x, ldx, lane, mask);
+        return;
+    }
+    constexpr int PB = (8 / (R * C)) >= 1 ? (8 / (R * C)) : 1;
+    const int64_t sl = len <= cuts.z ? cuts.y : cuts.w;
+    const int64_t segs = (len + sl - 1) / sl;
+#pragma unroll
+    for (int c = 0; c < C; ++c) acc[c] = f4zero();
+    for (int64_t s0 = 0; s0 < segs; s0 += PB) {
+        for (int q = 0; q < PB; ++q) {
+            float4 pv[C];
+            if (s0 + q < segs) {
+                const int64_t sb = b + (s0 + q) * sl;
+                fold_walk<G, C, R>(pv, idx, sb, sb + sl < e ? sb + sl : e, w, x, ldx, lane, mask);
+            } else {
+#pragma unroll
+                for (int c = 0; c < C; ++c) pv[c] = f4zero();
+            }
+#pragma unroll
+            for (int c = 0; c < C; ++c) acc[c] = add4(acc[c], pv[c]);
+        }
+    }
+}
+
+template <int G, int C>
+__global__ void __launch_bounds__(256, 2) fold_users_kernel(const int64_t* __restrict__ indptr, const int64_t* __restrict__ indices,
+                                                         const int64_t* __restrict__ users, const float* __restrict__ wq, int64_t n,
+                                                         const float* __restrict__ u0, int64_t ldu0, const mmssl_fold_tables_t t,
+                                                         int K, float inv_layers, float rate, const int4 cuts,
+                                                         float* __restrict__ out, int64_t ldo) {
+    pdl_wait();
+    extern __shared__ float4 fold_sm[];                     // [Q][K + 2][C][G] float4: each table's row, in the lane layout
+    constexpr int D4 = G * C;
+    const int T = K + 2;
+    const int grp = threadIdx.x / G, lane = threadIdx.x & (G - 1);
+    const unsigned mask = group_mask<G>();
+    const int ql = grp / T, tab = grp - ql * T;
+    const int64_t q = (int64_t)blockIdx.x * (blockDim.x / (G * T)) + ql;
+    const bool live = q < n;
+    float4* row_sm = fold_sm + (int64_t)grp * D4;
+    if (live) {
+        const int64_t b = indptr[q], e = indptr[q + 1];
+        const float w = wq[q];
+        float4 acc[C];
+        if (tab < K) {
+            const float* x = t.layer[0];
+            int64_t ldx = t.ld_layer[0];
+#pragma unroll
+            for (int k = 1; k < MMSSL_FOLD_MAX_LAYERS; ++k)         // selected, not indexed: the descriptor stays in parameter space
+                if (k == tab) { x = t.layer[k]; ldx = t.ld_layer[k]; }
+            fold_sum<G, C, 1>(acc, indices, b, e, w, x, ldx, cuts, lane, mask);
+            if (tab == K - 1) {                             // spmm_item's softmax epilogue (the last GCN layer)
+                float m = -INFINITY;
+#pragma unroll
+                for (int c = 0; c < C; ++c) m = fmaxf(m, max4(acc[c]));
+                m = group_max<G>(m, mask);
+                float sum = 0.f;
+#pragma unroll
+                for (int c = 0; c < C; ++c) {
+                    acc[c].x = __expf(acc[c].x - m); acc[c].y = __expf(acc[c].y - m);
+                    acc[c].z = __expf(acc[c].z - m); acc[c].w = __expf(acc[c].w - m);
+                    sum += (acc[c].x + acc[c].y) + (acc[c].z + acc[c].w);
+                }
+                sum = group_sum<G>(sum, mask);
+                const float inv = 1.f / sum;
+#pragma unroll
+                for (int c = 0; c < C; ++c) acc[c] = scale4(acc[c], inv);
+            }
+        } else {
+            fold_sum<G, C, 2>(acc, indices, b, e, w, tab == K ? t.xv : t.xt, tab == K ? t.ldxv : t.ldxt, cuts, lane, mask);
+        }
+#pragma unroll
+        for (int c = 0; c < C; ++c) row_sm[c * G + lane] = acc[c];
+    }
+    __syncthreads();
+    if (!live || tab != 0) return;
+    // the forward's order: S = u_0 + u_1 (SpMM s_mode 2), S += u_{k+1} (s_mode 1); K = 0: S = 1 * u_0 (axpby)
+    const int64_t u = users != nullptr ? users[q] : -1;
+    float4 s[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) s[c] = u >= 0 ? ld4(u0 + u * ldu0 + lane * 4 + c * (4 * G)) : f4zero();
+    const float4* qsm = fold_sm + (int64_t)ql * T * D4;
+    if (K == 0) {
+#pragma unroll
+        for (int c = 0; c < C; ++c) s[c] = scale4(s[c], 1.f);
+    }
+    for (int k = 0; k < K; ++k)
+#pragma unroll
+        for (int c = 0; c < C; ++c) s[c] = add4(s[c], qsm[k * D4 + c * G + lane]);
+    // combine_fwd_kernel's arithmetic
+    float4 av[C], bv[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+        av[c] = qsm[K * D4 + c * G + lane];
+        bv[c] = qsm[(K + 1) * D4 + c * G + lane];
+    }
+    const float sa = row_dot<G, C>(av, av, mask);
+    const float sb = row_dot<G, C>(bv, bv, mask);
+    const float ia = rate / fmaxf(sqrtf(sa), kNormEps);
+    const float ib = rate / fmaxf(sqrtf(sb), kNormEps);
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+        s[c] = scale4(s[c], inv_layers);
+        fma4(s[c], ia, av[c]);
+        fma4(s[c], ib, bv[c]);
+        st4(out + q * ldo + lane * 4 + c * (4 * G), s[c]);
+    }
+}
+
 // ---- plain element-wise passes over strided [n, d] matrices (d % 4 == 0) ----
 __global__ void axpby_kernel(const float* __restrict__ x, int64_t ldx, int64_t n, int d4, float alpha,
                              const float* __restrict__ alpha_dev, float beta, float* __restrict__ y, int64_t ldy) {
@@ -391,6 +548,39 @@ extern "C" int mmssl_unit_rows(const float* x, int64_t ldx, int64_t n, int d, fl
     if (n == 0) return 0;
     return dispatch_width(d, [&](auto G, auto C) {
         MMSSL_CUDA_LAUNCH((unit_rows_kernel<decltype(G)::value, decltype(C)::value>), dim3(row_blocks(n, decltype(G)::value)), dim3(256), 0, st, x, ldx, n, out, ldo);
+        MMSSL_LAUNCH_OK();
+        return 0;
+    }, __func__);
+}
+
+extern "C" int mmssl_fold_users(const int64_t* indptr, const int64_t* indices, const int64_t* users, const float* w, int64_t n,
+                                const float* u0, int64_t ldu0, const mmssl_fold_tables_t* tables, int d, int n_layers,
+                                float inv_layers, float rate, float* out, int64_t ldo, void* stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    MMSSL_REQUIRE(tables != nullptr && n >= 0, "null tables or negative n");
+    if (n_layers < 0 || n_layers > MMSSL_FOLD_MAX_LAYERS) {
+        snprintf(last_error_buffer(), 512, "mmssl_fold_users: %d GCN layers; the kernel is built for 0 to %d", n_layers,
+                 MMSSL_FOLD_MAX_LAYERS);
+        return 1;
+    }
+    if (!width_supported(d)) return fail_width(__func__, d);
+    const mmssl_fold_tables_t t = *tables;
+    for (int k = 0; k < n_layers; ++k) MMSSL_REQUIRE(t.layer[k] != nullptr && ROW_ALIGN_OK(t.layer[k], t.ld_layer[k]), "layer table alignment");
+    MMSSL_REQUIRE(t.xv != nullptr && t.xt != nullptr && ROW_ALIGN_OK(t.xv, t.ldxv) && ROW_ALIGN_OK(t.xt, t.ldxt), "Xv / Xt alignment");
+    MMSSL_REQUIRE(ROW_ALIGN_OK(out, ldo) && (u0 == nullptr || ROW_ALIGN_OK(u0, ldu0)), "alignment");
+    MMSSL_REQUIRE(u0 != nullptr || users == nullptr, "user ids need the u_0 table");
+    MMSSL_REQUIRE(indptr != nullptr && w != nullptr && (n == 0 || out != nullptr), "null argument");
+    if (n == 0) return 0;
+    const int4 cuts = spmm_plan_cuts();
+    return dispatch_width(d, [&](auto G, auto C) {
+        constexpr int g = decltype(G)::value, c = decltype(C)::value;
+        const int per_query = g * (n_layers + 2);
+        const int q_per_cta = 256 / per_query;           // >= 1: (MMSSL_FOLD_MAX_LAYERS + 2) * 32 <= 256
+        const int64_t blocks = (n + q_per_cta - 1) / q_per_cta;
+        MMSSL_REQUIRE(blocks <= 0x7fffffffll, "too many queries for one launch");
+        const size_t smem = sizeof(float4) * (size_t)q_per_cta * (n_layers + 2) * g * c;
+        MMSSL_CUDA_LAUNCH((fold_users_kernel<g, c>), dim3((unsigned)blocks), dim3(q_per_cta * per_query), smem, st, indptr, indices,
+                          users, w, n, u0, ldu0, t, n_layers, inv_layers, rate, cuts, out, ldo);
         MMSSL_LAUNCH_OK();
         return 0;
     }, __func__);

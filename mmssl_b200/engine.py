@@ -61,6 +61,8 @@ class FwdState:
     i_last: Optional[torch.Tensor] = None
     sumsq_u: Optional[torch.Tensor] = None  # per-block sum(Uv^2+Ut^2) / (Iv^2+It^2) for feat_reg
     sumsq_i: Optional[torch.Tensor] = None
+    u0: Optional[torch.Tensor] = None       # keep_fold: the user id rows after the id fusion (u_0) ...
+    i_layers: Optional[tuple] = None        # ... and the item layer tables i_0 .. i_{K-1} the user layers gather (foldin.py)
 
 
 # The branches of the step and the priority of each one's stream (0 = lowest .. -5): the item-side twin of the critical id / GCN
@@ -238,10 +240,12 @@ class Engine:
 
     # ------------------------------------------------------------------ forward
     def forward(self, P: Dict[str, torch.Tensor], feats: Tuple[FeatureStore, FeatureStore],
-                graphs: Sequence[BipartiteGraph], masks, want_sumsq: bool = True, side_pre=None):
+                graphs: Sequence[BipartiteGraph], masks, want_sumsq: bool = True, side_pre=None, keep_fold: bool = False):
         """masks: None, a pair of [I, d] keep-masks (0 or 1/(1-p)), or a callable returning one -- the
         callable and `side_pre` run on a branch forked at the head of the modality branch, i.e. off the critical path: the
-        projection GEMM starts at once, and only its epilogues (which apply the masks) wait for that branch."""
+        projection GEMM starts at once, and only its epilogues (which apply the masks) wait for that branch.
+        keep_fold: the returned state also holds u_0 and the item layer tables i_0 .. i_{K-1} (references to tables the forward
+        computes anyway: the same kernels and launches), which with X2 are what a user row is folded from (foldin.py)."""
         g_ui, g_iu, g_vui, g_viu, g_tui, g_tiu = graphs
         U, I = g_ui.shape
         d, K = self.d, self.K
@@ -302,6 +306,8 @@ class Engine:
         # the layer sums S_u, S_i accumulate in the SpMM epilogue (:213-214)
         s_u, s_i = self._new(U, d, dev=dev), self._new(I, d, dev=dev)
         cur_i = i0
+        if keep_fold:
+            st.u0, st.i_layers = u0, ()
         if K == 0:
             ops.axpby(u0, 1.0, 0.0, s_u)
             ops.axpby(i0, 1.0, 0.0, s_i)
@@ -309,6 +315,8 @@ class Engine:
             last = k == K - 1
             epi = ops.EPI_SOFTMAX if last else ops.EPI_NONE
             mode = 2 if k == 0 else 1
+            if keep_fold:
+                st.i_layers += (cur_i,)
             u_n = self._spmm(g_ui, "fwd", [cur_i], "i", epilogue=epi, ss=[s_u], s_mode=mode, sbases=[u0] if k == 0 else None)[0]
             i_n = self._spmm(g_iu, "fwd", [u_n], "u", epilogue=epi, ss=[s_i], s_mode=mode, sbases=[i0] if k == 0 else None)[0]
             if last:

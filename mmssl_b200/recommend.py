@@ -36,7 +36,7 @@ from .parallel import RowPartition, all_gather_rows
 EXCLUDE = ("train", "seen")
 FILES = ("ids", "scores", "users")
 FORMAT = "mmssl_b200.recommend.v1"
-QUERY_FILES = ("users", "items")            # the row-id file of a recommendation / a similar-items (similar.py) export
+QUERY_FILES = ("users", "items", "queries")   # the row-id file of a recommendation / similar-items or audience / fold-in export
 MANIFEST = "manifest.json"
 _RANK_MANIFEST = re.compile(r"rank(\d{5})-of-(\d{5})\.json")
 
@@ -362,7 +362,8 @@ def _load_set(out_dir: str, prefix: str, meta: dict, query: str = "users"):
 # the readers of the export formats that share the file logic above: a directory of one kind is refused by the other's reader
 READERS = {FORMAT: "recommendations (mmssl_b200.recommend.read)",
            "mmssl_b200.similar.v1": "similar items (mmssl_b200.similar.read)",
-           "mmssl_b200.audience.v1": "audiences (mmssl_b200.audience.read)"}
+           "mmssl_b200.audience.v1": "audiences (mmssl_b200.audience.read)",
+           "mmssl_b200.foldin.v1": "fold-in recommendations (mmssl_b200.foldin.read)"}
 
 
 def _check_format(out_dir: str, meta: dict, fmt: str) -> None:

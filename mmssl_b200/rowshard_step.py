@@ -493,6 +493,19 @@ class RowShardedHotStep:
         self.n_gathers, self.gathered_bytes, self.n_reduce_scatters = counters
         return outs[0], outs[1]
 
+    def fold_tables(self) -> Dict[str, object]:
+        """Collective, under ``final_embeddings``' rules.  What a user row is folded from (foldin.ShardedFoldIn): the rank's padded
+        blocks of the eval-mode forward's u_0 ("u0", the id rows after the id fusion), item layer tables i_0 .. i_{K-1}
+        ("layers"), projections ("xv", "xt") and final item table ("i_f"), fresh tensors or the live parameters where the forward
+        uses them as they are (u_0 = E_u, i_0 = E_i without modality graphs)."""
+        counters = (self.n_gathers, self.gathered_bytes, self.n_reduce_scatters)
+        self._quiesce()
+        outs, st = self.engine.forward(self.P, self.feats, self.graphs, None, want_sumsq=False, keep_fold=True)
+        self._quiesce()
+        self.n_gathers, self.gathered_bytes, self.n_reduce_scatters = counters
+        d = self.cfg.embed_size
+        return dict(u0=st.u0, layers=st.i_layers, xv=st.X2[:, :d], xt=st.X2[:, d:], i_f=outs[1])
+
     def projections(self) -> Tuple[torch.Tensor, torch.Tensor]:
         """The eval-mode modality projections Xv = Fv Wv^T + bv, Xt = Ft Wt^T + bt (Models.py:173-174, no dropout) of the rank's
         padded [block, d] item rows, fresh tensors.  Row-local, so no collective: the rank's feature rows and the replicated

@@ -247,6 +247,31 @@ class Trainer:
         projected with the trained weights, in space "image" or "text"."""
         return self.similar(k, space).topk_features(image_feats, text_feats)
 
+    _held = None                                      # (train, val, test) host CSRs of the users, built on first use
+
+    def fold(self):
+        """foldin.FoldIn over the eval-mode forward ``test`` and ``recommender`` run (the full step's current modality graphs),
+        with the training, validation and test rows of the trained users for exclude="train" / "seen"."""
+        from .dataset import held_csr
+        from .foldin import FoldIn
+        if self._held is None:
+            d = self.data
+            self._held = tuple(held_csr(rows, self.n_users) for rows in (d.train_items, d.val_set, d.test_set))
+        hs = self.step.hs
+        return FoldIn.from_forward(hs.engine, hs.P, hs.feats, hs.graphs, self._held)
+
+    def fold_in(self, rows, users=None):
+        """[n, d] fp32 on the device: the final user row of each query -- an item list (``rows``, an (indptr, indices) host
+        pair), with the id of a trained user (``users``) or -1 for a user the model never trained on -- with the trained item
+        side held fixed (foldin.py).  A trained user's own training row gives the forward's user row."""
+        return self.fold().fold(rows, users)
+
+    def recommend_for(self, rows, k: int, users=None, exclude: str = "train"):
+        """The top-k items of each folded query (fold_in): (ids [n, k] int64, scores [n, k] fp32) on the device, -1 past the end
+        of a short list.  The query's items are never listed; for a trained user "train" also masks its training items (so its
+        own training row gives ``recommend``'s list), "seen" also its validation and test items."""
+        return self.fold().topk(rows, k, users, exclude)
+
     def sample(self):
         if self.sampler == "device":
             self._dev_sampler.sample_into(self._triples, step=self._n_sampled)

@@ -16,8 +16,15 @@
         block): of every item, or of the int64 item ids in FILE (.npy).  --exclude drops the users who had the item in training
         ("train") or also in val / test ("seen"); --chunk then counts items.
 
-``recommend.read(DIR)`` returns (users, ids, scores) of either layout, ``audience.read(DIR)`` (items, ids, scores).  Prints one JSON
-line (rank 0)."""
+    --fold-in FILE.npz: in either mode, export the top-k items of users given by item lists instead (mmssl_b200/foldin.py): FILE
+        holds ``indptr`` / ``indices`` (int64, one row of item ids per query) and optionally ``users`` (int64, the id of a trained
+        user, or -1 for a user the model never trained on).  Writes DIR/{ids,scores,queries}.npy, ``queries`` = each list's row
+        number in FILE.  Row-sharded: a rank takes the queries of the users of its block plus its contiguous share of the
+        new-user queries and writes rankRRRRR-of-WWWWW.*.  --exclude adds the training ("train") or also the val / test ("seen")
+        items of a trained user to the query's own; --chunk then counts queries.
+
+``recommend.read(DIR)`` returns (users, ids, scores) of either layout, ``audience.read(DIR)`` (items, ids, scores),
+``foldin.read(DIR)`` (queries, ids, scores).  Prints one JSON line (rank 0)."""
 import argparse
 import json
 import os
@@ -30,11 +37,22 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
-from mmssl_b200 import audience, checkpoint, recommend  # noqa: E402
+from mmssl_b200 import audience, checkpoint, foldin, recommend  # noqa: E402
 
 
 def _items(a, n_items: int) -> np.ndarray:
     return np.load(a.items).astype(np.int64).reshape(-1) if a.items else np.arange(n_items, dtype=np.int64)
+
+
+def _fold_queries(path: str):
+    """((indptr, indices), users) of a --fold-in file; users -1 where the file has none."""
+    with np.load(path) as f:
+        rows = (f["indptr"].astype(np.int64), f["indices"].astype(np.int64))
+        n = rows[0].size - 1
+        users = f["users"].astype(np.int64).reshape(-1) if "users" in f.files else np.full(n, -1, np.int64)
+    if users.size != n:
+        raise SystemExit(f"{path}: {users.size} users for {n} query rows")
+    return rows, users
 
 
 def load_trainer(a, dev):
@@ -57,6 +75,10 @@ def load_trainer(a, dev):
 
 def one_gpu(a, dev):
     t = load_trainer(a, dev)
+    if a.fold_in:
+        rows, users = _fold_queries(a.fold_in)
+        n = t.fold().export(rows, a.k, a.out, users, a.exclude, chunk=a.chunk)
+        return dict(queries=n, users=t.n_users, items=t.n_items)
     if a.audience:
         aud, item_table = t.audience_ranker(a.k, a.exclude)         # what Trainer.audience ranks with
         n = aud.export(item_table, _items(a, t.n_items), a.out, chunk=a.chunk)
@@ -68,6 +90,13 @@ def one_gpu(a, dev):
 
 def load_sharded(a, dev, rank, world):
     """(the rank's ShardedDataset, its padded blocks of the final user and item tables) of the row-sharded checkpoint."""
+    sh, step = load_sharded_step(a, dev, rank, world)
+    u_f, i_f = step.final_embeddings()
+    return sh, u_f, i_f
+
+
+def load_sharded_step(a, dev, rank, world):
+    """(the rank's ShardedDataset, its RowShardedHotStep with the checkpoint loaded)."""
     from mmssl_b200.dataset import ShardedDataset
     from mmssl_b200.engine import P_EI, P_EU
     from mmssl_b200.hotstep import HotStepConfig
@@ -89,11 +118,32 @@ def load_sharded(a, dev, rank, world):
     step = RowShardedHotStep(Pl, fl, gl, cfg, B, pu, pi, rank)
     del st, P
     step.load(a.sharded)
-    u_f, i_f = step.final_embeddings()
-    return sh, u_f, i_f
+    return sh, step
+
+
+def fold_share(users: np.ndarray, part_u, rank: int) -> np.ndarray:
+    """Row numbers of the --fold-in queries rank `rank` folds: those of the users of its block, then its contiguous share of the
+    new-user (-1) queries, each in file order."""
+    own = np.nonzero((users >= 0) & (users // part_u.block == rank))[0]
+    new = np.nonzero(users < 0)[0]
+    lo, hi = (new.size * rank) // part_u.world, (new.size * (rank + 1)) // part_u.world
+    return np.concatenate([own, new[lo:hi]])
+
+
+def sharded_fold_in(a, dev, rank, world):
+    sh, step = load_sharded_step(a, dev, rank, world)
+    rows, users = _fold_queries(a.fold_in)
+    if users.size and int(users.max()) >= sh.n_users:
+        raise SystemExit(f"{a.fold_in}: a user id outside [0, {sh.n_users})")
+    fi = foldin.ShardedFoldIn.from_dataset(step.fold_tables(), sh, a.model_cat_rate)
+    pick = fold_share(users, sh.part["user"], rank)
+    n = fi.export(foldin.take_rows(rows, pick), a.k, a.out, users[pick], a.exclude, chunk=a.chunk, names=pick)
+    return dict(queries=int(rows[0].size - 1), users=sh.n_users, items=sh.n_items, rows_written_by_rank0=n)
 
 
 def sharded(a, dev, rank, world):
+    if a.fold_in:
+        return sharded_fold_in(a, dev, rank, world)
     sh, u_f, i_f = load_sharded(a, dev, rank, world)
     if a.audience:
         aud = audience.ShardedAudience.from_shards(sh, a.k, a.exclude, device=dev)
@@ -116,6 +166,7 @@ def main(argv=None):
     ap.add_argument("--chunk", type=int, default=1 << 16, help="users (items with --audience) ranked per launch (bounds the device memory)")
     ap.add_argument("--audience", action="store_true", help="export the top-k users of items instead of the top-k items of users")
     ap.add_argument("--items", help="with --audience: a .npy of the item ids to rank (default: every item)")
+    ap.add_argument("--fold-in", help="a .npz of query rows (indptr, indices, optional users): export their top-k items instead")
     # both rates shape the eval-mode forward and neither checkpoint kind stores them: give the trained run's values
     ap.add_argument("--id-cat-rate", type=float, default=0.36, help="the run's id_cat_rate (not in its checkpoint; default 0.36)")
     ap.add_argument("--model-cat-rate", type=float, default=0.55, help="the run's model_cat_rate (not in its checkpoint; default 0.55)")
@@ -124,6 +175,8 @@ def main(argv=None):
         ap.error("give DATA --checkpoint FILE, or --sharded DIR --shards DIR")
     if a.items and not a.audience:
         ap.error("--items needs --audience")
+    if a.fold_in and a.audience:
+        ap.error("--fold-in and --audience are two different exports: give one")
     rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
